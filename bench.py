@@ -1,7 +1,7 @@
 #!/usr/bin/env python
-"""bench.py -- views/sec of the IGGT multi-view forward on B200 (BASELINE.json metric).
+"""bench.py -- views/sec of the IGGT multi-view forward on H100 (BASELINE.json metric).
 
-  python bench.py [--gpus N] [--steps K] [--warmup W] [--impl b200|reference]
+  python bench.py [--gpus N] [--steps K] [--warmup W] [--impl b200|reference] [--dump-outputs DIR]
 
 Workload (config C2 of BASELINE.json): one synthetic scene of 8 views at 518x518, random-init weights of the
 reference architecture, fp16 trunk operands (fp32 accumulate / residual / LayerNorm), every output the
@@ -18,9 +18,12 @@ pinned-host -> device copy of the images and the device -> host copy of every pr
 `--impl reference` times the reference algorithm's CPU implementation (the oracle port, all host threads) on a
 bounded sample of the same workload: `--ref-views` (default 1) of the views per step at the same resolution - its
 `config` says so (`views_per_step`), its global attention spans that many views only.
+`--dump-outputs DIR` writes what the timed path returned in its last timed step as DIR/<name>.npy (float32; inputs and
+weights are seeded, so two builds can be compared output for output).
 """
 import argparse
 import json
+import math
 import os
 import subprocess
 import sys
@@ -45,7 +48,7 @@ def measured_peaks():
         d = json.load(open(p))
         return {"tflops": d.get("bf16_tflops_sustained", d.get("bf16_tflops")), "gbs": d.get("hbm_gbs"),
                 "source": "MEASURED_PEAKS.json (sustained cuBLAS bf16 / stream copy)"}
-    return {"tflops": 1400.0, "gbs": 6650.0, "source": "fallback (B200_PROFILING.md)"}
+    return {"tflops": 989.0, "gbs": 3350.0, "source": "NVIDIA H100 SXM data sheet (dense fp16, HBM3; 700 W card)"}
 
 
 class ClockSampler:
@@ -150,7 +153,7 @@ def workload_config(args, world):
             "scenes": args.scenes, "views": args.views, "image": [args.size, args.size],
             "weights": "random-init, reference architecture (1.30 B params)",
             "parallelism": f"view-shard x{world}" if world > 1 else "single GPU",
-            "l2": "per-step working set (2.6 GB 16-bit weights + activations) >> 126 MB L2: no flush needed"}
+            "l2": "per-step working set (2.6 GB 16-bit weights + activations) >> 50 MB L2: no flush needed"}
 
 
 # ------------------------------------------------------------------------------------------- our arm
@@ -220,6 +223,8 @@ def run_b200(args):
     e1.record()
     barrier()
     ms = e0.elapsed_time(e1) / args.steps
+    if args.dump_outputs and rank == 0:
+        dump_outputs(out, args.dump_outputs)
     launches = (ops.STATS["launches"] - launches0) // args.steps
     if graphed:                                    # replays bypass the Python counter: count one eager forward
         c0 = ops.STATS["launches"]
@@ -277,21 +282,13 @@ def run_b200(args):
     roof.update({"launches_per_step": d["n"] // 2, "avg_launch_ms": d["ms"] / d["n"], "share_of_step": d["ms"] / total_ms,
                  "peak_source": peaks["source"]})
     if name == "iggt_attention_fwd":
-        # head_dim 64 attention is bounded by the exp unit (MUFU: 16 ex2/clk/SM measured, scripts/ubench/mufu.cu) before
-        # the tensor pipe: 1 exp per 256 tensor FLOPs -> at most 0.5 of the tensor peak.  Report that roofline too.
-        clk = (clocks or {}).get("sm_mhz") or 1965.0
+        # head_dim 64 attention also needs the exp unit (MUFU: 16 ex2/clk/SM) next to the tensor pipe: 1 exp per 256
+        # tensor FLOPs.  Report that roofline too.
+        clk = (clocks or {}).get("sm_mhz") or 1980.0
         exps = d["flops"] / 256.0
-        peak_exp = 16.0 * 148 * clk * 1e6
+        peak_exp = 16.0 * torch.cuda.get_device_properties(dev).multi_processor_count * clk * 1e6
         roof["mufu_roofline"] = {"achieved_gexp_s": exps / (d["ms"] * 1e-3) / 1e9, "peak_gexp_s": peak_exp / 1e9,
-                                 "frac": exps / (d["ms"] * 1e-3) / peak_exp,
-                                 "note": "ncu (profiles/r02a_ncu_all_kernels.csv): sm__inst_executed_pipe_xu 75.7 % (global), 55.1 % (frame) of peak; the softmax warps are latency-bound, not MUFU-bound (profiles/r02b_attn_sweep.json)"}
-        tp = os.path.join(ROOT, "profiles", "r02_ncu_traffic.json")
-        if os.path.exists(tp) and world == 1 and args.views == 8 and args.size == 518:
-            t = json.load(open(tp))["iggt_attention_fwd"]
-            # per launch, averaged over the 24 global + 48 frame launches of a step
-            roof["traffic"] = (24 * t["global_c2_bytes_per_launch"] + 48 * t["frame_c2_bytes_per_launch"]) / 72
-            roof["traffic_unit"] = "bytes per launch (dram read+write, ncu --set full)"
-            roof["algorithmic_bytes_per_launch"] = d["bytes"] / d["n"]
+                                 "frac": exps / (d["ms"] * 1e-3) / peak_exp}
     shares = {k: {"share": v["ms"] / total_ms, "ms_per_step": v["ms"] / 2, "n_per_step": v["n"] // 2,
                   "tflops": (v["flops"] / (v["ms"] * 1e-3) / 1e12) if v["flops"] else None,
                   "gbs": v["bytes"] / (v["ms"] * 1e-3) / 1e9}
@@ -361,7 +358,7 @@ def cpu_threads():
 
 
 def gpu_eager_baseline(args, dt, images_dev):
-    """SURVEY 8(d)'s "real bar": the reference algorithm as PyTorch eager on THIS B200 - the oracle port with its
+    """SURVEY 8(d)'s "real bar": the reference algorithm as PyTorch eager on THIS GPU - the oracle port with its
     Linear / SDPA calls issued natively in the autocast dtype (ref_model.NATIVE_16BIT: cuBLAS 16-bit GEMMs, the
     SDPA backend torch picks; heads fp32 with cuDNN TF32 convolutions, PyTorch's default), same inputs and config."""
     from oracle import ref_model, weights  # checker used as a baseline (never on the product path)
@@ -392,6 +389,30 @@ def gpu_eager_baseline(args, dt, images_dev):
             "what": f"oracle port as PyTorch {torch.__version__} eager on the same GPU: {args.dtype} Linear / SDPA "
                     "(cuBLAS + torch's SDPA backend), fp32 LayerNorm / residual, heads fp32 with cuDNN TF32 convolutions; "
                     f"{reps} forwards after 1 warm-up, CUDA events; device-resident inputs"}
+
+
+DUMP_BUDGET = 63_000_000      # bytes of float32 written by --dump-outputs in all (64 MB with headers to spare)
+
+
+def dump_outputs(out, path):
+    """The arrays a caller of the timed forward receives, as float32 `path/<name>.npy`.  An output whose share of the
+    64 MB budget is too small is replaced by a fixed sample of its flattened elements (indices from a seeded generator,
+    sorted, so the same shape always gives the same sample)."""
+    import numpy as np
+    arrays = {}
+    for k, v in out.items():
+        if isinstance(v, (list, tuple)):
+            v = torch.stack(list(v))
+        if torch.is_tensor(v):
+            arrays[k] = v.detach().float().cpu().numpy()
+    total = sum(a.size for a in arrays.values())
+    os.makedirs(path, exist_ok=True)
+    for k, a in sorted(arrays.items()):
+        keep = a.size if total * 4 <= DUMP_BUDGET else max(1, math.floor(a.size * DUMP_BUDGET / (total * 4)))
+        if keep < a.size:
+            idx = np.sort(np.random.default_rng(0).choice(a.size, size=keep, replace=False))
+            a = a.reshape(-1)[idx]
+        np.save(os.path.join(path, f"{k}.npy"), np.ascontiguousarray(a, dtype=np.float32))
 
 
 def cpu_baseline(args):
@@ -425,13 +446,15 @@ def main():
     ap.add_argument("--ref-views", type=int, default=1, help="views per step of the CPU legs (bounded sample)")
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-graph", action="store_true", help="launch kernels eagerly instead of replaying a CUDA graph")
-    ap.add_argument("--quick", action="store_true", help="profiling mode: warm-up + steps only (run this under ncu)")
+    ap.add_argument("--quick", action="store_true", help="profiling mode: warm-up + steps only (run this under a profiler)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the outputs of the last timed step as DIR/<name>.npy (float32, at most 64 MB in all)")
     args = ap.parse_args()
     if args.impl == "reference":
         run_reference(args)
     else:
         if not torch.cuda.is_available():
-            raise SystemExit("bench.py needs a CUDA device (there is no CPU fallback for the B200 path)")
+            raise SystemExit("bench.py needs a CUDA device (there is no CPU fallback for the GPU path)")
         run_b200(args)
 
 

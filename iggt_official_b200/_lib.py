@@ -99,7 +99,7 @@ class CameraWeights(ctypes.Structure):
 
 
 def build(verbose: bool = False) -> str:
-    """Compile every CUDA source for sm_100a (nvcc cross-compiles without a GPU)."""
+    """Compile every CUDA source for sm_90a (nvcc cross-compiles without a GPU)."""
     cmd = ["make", "-C", CSRC_DIR, "-j", str(min(16, os.cpu_count() or 4))]
     res = subprocess.run(cmd, capture_output=True, text=True)
     if res.returncode != 0:

@@ -1,22 +1,15 @@
-// Flash-attention forward for head_dim 64 on sm_100a (third generation of this kernel; the first two are in the git
-// history).  Replaces F.scaled_dot_product_attention at iggt/layers/attention.py:61-66.
+// Flash-attention forward for head_dim 64 on sm_90a.  Replaces F.scaled_dot_product_attention at
+// iggt/layers/attention.py:61-66.
 //
-// Persistent CTAs over work items (sequence, head, pair of 128-row query tiles A / B), 20 warps:
-//   WG0     : warp 0 TMA producer (Q double-buffered per tile, 3-stage K / V ring shared by both tiles),
-//             warps 1 and 3 one tcgen05.mma issuer thread per query tile, warp 2 TMEM allocator   (setmaxnreg.dec)
-//   WG1,WG2 : softmax of query tile A, each thread owns HALF a query row (64 of the 128 keys of a kv tile)
-//   WG3,WG4 : softmax of query tile B                                                               (setmaxnreg.inc)
-// Four softmax warps per SM sub-partition hide the mbarrier / TMEM / MUFU latencies that left the second generation
-// (two per sub-partition) at 50 % of the MUFU roofline (profiles/r01_ncu_notes.md).
-// O accumulates in TMEM across kv tiles (tcgen05.mma accumulate); the running max is only refreshed -- and O
-// rescaled in TMEM (tcgen05.ld / tcgen05.st) -- when some row's max grows by more than 2^8 (lazy rescaling), so the
-// steady-state loop is: TMEM->reg S, max, scale-and-shift (packed FFMA2), exp2 (MUFU), row sums (packed FADD2), pack
-// to 16 bit, tcgen05.st P.  P never touches shared memory: the PV MMA reads its A operand from TMEM (PT variant, the
-// default).  Row halves agree on the max through a shared-memory exchange that only happens on a rescale; the
-// decision is taken with one bar.red.or per tile.  Item schedule: Attn3Items below.
-//
-// TMEM map (512 columns): S_A [0,128)  S_B [128,256)  O_A [256,320)  O_B [320,384)  P_A [384,448)  P_B [448,512)
-// (P: 128 keys x 16 bit = 64 columns per query row)
+// Persistent CTAs over work items (sequence, head, pair of 128-row query tiles A / B), 3 warpgroups:
+//   WG0      : warp 0 TMA producer (Q double-buffered per tile, a K / V ring shared by both tiles)
+//   WG1, WG2 : one consumer per query tile (A, B), each working its 128 rows as two 64-row halves
+// For every kv tile and half, a consumer computes S = Q K^T (wgmma, both operands from 128B-swizzled shared memory,
+// fp32 in registers), runs the online softmax on the register fragment (row max / sum across the 4 threads of a row),
+// packs P to 16 bit straight into the A-operand registers of O += P V (wgmma with A from registers, V read MN-major
+// from shared memory) and keeps O in registers.  The two consumers interleave their softmax phases with each other's
+// MMAs.
+// Item schedule: Attn3Items below.
 #include <stdlib.h>
 #include "ptx.cuh"
 #include "tmap.cuh"
@@ -28,15 +21,11 @@ namespace iggt {
 constexpr int A3_BQ = 128;
 constexpr int A3_BK = 128;
 constexpr int A3_D = 64;
-constexpr int A3_STAGES = 3;
-constexpr int A3_THREADS = 640;
+constexpr int A3_STAGES = 4;
+constexpr int A3_THREADS = 384;
 constexpr int A3_TILE = A3_BK * A3_D * 2;     // 16 KB
-constexpr int A3_P = A3_BQ * A3_BK * 2;       // 32 KB
-constexpr int A3_XCHG = 2 * 2 * 128 * 4;      // max / sum exchange: [tile][half][row] fp32
-constexpr int A3_SMEM = A3_TILE * (4 + 2 * A3_STAGES) + 2 * A3_P + A3_XCHG + 512;   // Q is double-buffered per tile
+constexpr int A3_SMEM = A3_TILE * (4 + 2 * A3_STAGES) + 512;   // Q is double-buffered per tile
 static_assert(A3_SMEM <= 232448, "shared memory budget");
-constexpr float A3_TAU = 8.0f;                // lazy-rescale threshold in log2 units
-constexpr int A3_DEFAULT_EMU8 = 0;            // probability pairs (of every 8) on the FMA-pipe exp2 by default
 
 struct Attn3Params {
   int Lq, Lk, H, num_seq;
@@ -45,9 +34,8 @@ struct Attn3Params {
   int64_t ldo;
   void* o;
   float scale_log2;
-  int stagger_at;       // tile A signals tile B's start after this many (x16) exps of its first kv tile (0..4)
   int light_tail;       // the last query pair of every (sequence, head) has no rows for tile B (Lq = 1374: 94 rows)
-  // split-KV (view-sharded ranks: 88 work items for 148 SMs): the kv tiles of every item are cut into `kv_splits` ranges
+  // split-KV (view-sharded ranks: 88 work items for 132 SMs): the kv tiles of every item are cut into `kv_splits` ranges
   // of `tiles_per_split`; each (item, split) writes its un-normalised fp32 O and (m, l) to the workspace and
   // attention3_merge_kernel combines the splits.  kv_splits == 1: the kernel writes the normalised 16-bit output itself.
   int kv_splits, tiles_per_split;
@@ -59,7 +47,7 @@ struct Attn3Params {
 // (Lq = 1374: 10.7 tiles) that pair is a half-weight item: tile B's MMAs and softmax are skipped outright for it, and
 // the static schedule is longest-processing-time-first - every CTA first takes its full items round-robin, then the
 // halves go (twice) to the CTAs that got one full item fewer, then round-robin again.  8 x 16 x (5 + 1/2) items on
-// 148 CTAs finish in 5.0 item-times instead of 6.0.  All roles of a CTA walk the same sequence.
+// 132 CTAs finish in 5.5 item-times instead of 6.0.  All roles of a CTA walk the same sequence.
 struct Attn3Items {
   int n_full, n_half, full_pairs, G, c, r;
   int k;          // position in this CTA's sequence
@@ -123,73 +111,7 @@ struct Attn3Items {
   }
 };
 
-__device__ __forceinline__ void tmem_st_32x32(uint32_t taddr, const uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x32.b32 [%0], "
-      "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, "
-      "%17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32};"
-      ::"r"(taddr), "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]),
-        "r"(r[8]), "r"(r[9]), "r"(r[10]), "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15]),
-        "r"(r[16]), "r"(r[17]), "r"(r[18]), "r"(r[19]), "r"(r[20]), "r"(r[21]), "r"(r[22]), "r"(r[23]),
-        "r"(r[24]), "r"(r[25]), "r"(r[26]), "r"(r[27]), "r"(r[28]), "r"(r[29]), "r"(r[30]), "r"(r[31])
-      : "memory");
-}
-__device__ __forceinline__ void tmem_st_wait() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
-
-// D[tmem] (+)= A[tmem] * B[smem desc]: A (M x K, 16-bit pairs packed per 32-bit column, lane = row) read from TMEM
-__device__ __forceinline__ void umma_f16_ts(uint32_t d_tmem, uint32_t a_tmem, uint64_t b_desc, uint32_t idesc,
-                                            uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, p;\n\t}\n" ::"r"(d_tmem),
-      "r"(a_tmem), "l"(b_desc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-
-// barrier + OR-reduction over `nthreads` threads of named barrier `id`
-__device__ __forceinline__ bool bar_red_or(uint32_t id, uint32_t nthreads, bool pred) {
-  uint32_t out;
-  asm volatile(
-      "{\n\t.reg .pred p, q;\n\t"
-      "setp.ne.u32 q, %3, 0;\n\t"
-      "bar.red.or.pred p, %1, %2, q;\n\t"
-      "selp.u32 %0, 1, 0, p;\n\t}\n"
-      : "=r"(out)
-      : "r"(id), "r"(nthreads), "r"(pred ? 1u : 0u)
-      : "memory");
-  return out != 0;
-}
-
-// 2^x for TWO values at once on the FMA / ALU pipes (no MUFU), with the sm_100 packed-fp32 instructions: Cody-Waite split
-// x = n + f with the 1.5 * 2^23 magic-number add (FADD2), f = x - n (FADD2 + FFMA2), a degree-3 polynomial for 2^f on
-// [-0.5, 0.5] (3 FFMA2, max relative error 1.0e-4 - below half an fp16 ulp of P), and the exponent patched in with one
-// shift-add per value.  5.5 issue slots per value against 1.5 for the MUFU path (the scale-and-shift FFMA2 is shared),
-// but the MUFU unit retires only 4 lanes / clk / sub-partition (8 clk per warp instruction): moving EMU8 of every 8
-// probability pairs here trades idle issue slots for MUFU time.  x may be -inf (masked keys): clamped to -126.
-__device__ __forceinline__ float2 ex2_emulated2(float2 x) {
-  x.x = fmaxf(x.x, -126.0f);
-  x.y = fmaxf(x.y, -126.0f);
-  const float2 magic = make_float2(12582912.0f, 12582912.0f);          // 1.5 * 2^23
-  const float2 t = fadd2(x, magic);                                      // low mantissa bits of t = round(x)
-  const float2 r = fadd2(t, make_float2(-12582912.0f, -12582912.0f));    // round(x), exact
-  const float2 f = ffma2(r, make_float2(-1.0f, -1.0f), x);               // x - round(x) in [-0.5, 0.5], exact
-  float2 pz = ffma2(make_float2(0.05583828315138817f, 0.05583828315138817f), f,
-                    make_float2(0.2426394820213318f, 0.2426394820213318f));
-  pz = ffma2(pz, f, make_float2(0.6931367516517639f, 0.6931367516517639f));
-  pz = ffma2(pz, f, make_float2(0.9999245405197144f, 0.9999245405197144f));
-  float2 y;
-  y.x = __int_as_float(__float_as_int(pz.x) + (__float_as_int(t.x) << 23));
-  y.y = __int_as_float(__float_as_int(pz.y) + (__float_as_int(t.y) << 23));
-  return y;
-}
-// which of the 32 probability pairs of a thread's 64 keys go through ex2_emulated2: EMU8 of every 8, evenly spread
-__host__ __device__ constexpr bool emu_pair(int pair, int emu8) {
-  return ((pair % 8) * emu8) / 8 != (((pair % 8) + 1) * emu8) / 8;
-}
-
-// PT: P goes to TMEM (tcgen05.st, consumed as the A operand of P V straight from tensor memory) instead of shared memory.
-template <bool BF16, int EMU8, bool PT>
+template <bool BF16>
 __global__ void __launch_bounds__(A3_THREADS, 1)
 attention3_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
                   const __grid_constant__ CUtensorMap tmV, const Attn3Params p) {
@@ -197,23 +119,13 @@ attention3_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant
   uint8_t* sQ = smem;                      // [2 buffers][2 tiles]: the next item's Q lands while this one runs
   uint8_t* sK = sQ + 4 * A3_TILE;
   uint8_t* sV = sK + A3_STAGES * A3_TILE;
-  uint8_t* sP = sV + A3_STAGES * A3_TILE;
-  float* xchg = reinterpret_cast<float*>(sP + 2 * A3_P);         // [2 tiles][2 halves][128]
-  uint64_t* bars = reinterpret_cast<uint64_t*>(reinterpret_cast<uint8_t*>(xchg) + A3_XCHG);
+  uint64_t* bars = reinterpret_cast<uint64_t*>(sV + A3_STAGES * A3_TILE);
   uint64_t* q_full = bars;                 // [2 buffers][2 tiles]
   uint64_t* q_empty = q_full + 4;          // [2 buffers][2 tiles]
-  uint64_t* k_full = q_empty + 4;          // [3]
+  uint64_t* k_full = q_empty + 4;          // [A3_STAGES]
   uint64_t* k_empty = k_full + A3_STAGES;
   uint64_t* v_full = k_empty + A3_STAGES;
   uint64_t* v_empty = v_full + A3_STAGES;
-  uint64_t* s_full = v_empty + A3_STAGES;  // [2]
-  uint64_t* s_empty = s_full + 2;
-  uint64_t* p_full = s_empty + 2;
-  uint64_t* p_empty = p_full + 2;
-  uint64_t* o_full = p_empty + 2;          // [2]  committed after every PV
-  uint64_t* o_free = o_full + 2;           // [2]  final O of an item has been read
-  uint64_t* stagger = o_free + 2;          // [1]  tile A is half-way through the exps of its first kv tile
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(stagger + 1);
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -227,28 +139,17 @@ attention3_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant
   }
   if (warp == 1 && lane == 0) {
     for (int i = 0; i < 4; ++i) { mbar_init(&q_full[i], 1); mbar_init(&q_empty[i], 1); }
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(&s_full[i], 1);   mbar_init(&s_empty[i], 256);
-      mbar_init(&p_full[i], 256); mbar_init(&p_empty[i], 1);
-      mbar_init(&o_full[i], 1);   mbar_init(&o_free[i], 256);
-    }
     for (int i = 0; i < A3_STAGES; ++i) {
-      mbar_init(&k_full[i], 1); mbar_init(&k_empty[i], 2);   // released by both tiles' MMA threads
+      mbar_init(&k_full[i], 1); mbar_init(&k_empty[i], 2);   // K / V: released by both consumers
       mbar_init(&v_full[i], 1); mbar_init(&v_empty[i], 2);
     }
-    mbar_init(stagger, 256);
     fence_barrier_init();
   }
-  if (warp == 2) tmem_alloc<512>(tmem_slot);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
   griddep_wait();
   griddep_launch();
 
   if (warp < 4) {
-    asm volatile("setmaxnreg.dec.sync.aligned.u32 56;");
     if (warp == 0 && lane == 0) {
       // ------------------------------------------------------------------ TMA producer
       int st = 0; uint32_t ph = 0;
@@ -288,260 +189,168 @@ attention3_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant
           if (j == j0 && has_next) load_q(nqp, nhead, nseq, nb);
         }
       }
-    } else if ((warp == 1 || warp == 3) && lane == 0) {
-      // ------------------------------------------------------------------ MMA issuers: one thread per query tile.
-      // The two tiles are independent pipelines (they only share the K/V stages), and tile B is started half a
-      // softmax period after tile A (`stagger`), so that the MUFU-heavy exp phase of one tile overlaps the
-      // TMEM-load / max / pack / st.shared phase of the other instead of both bursting on the MUFU unit at once.
-      const int t = warp == 1 ? 0 : 1;
-      constexpr uint32_t idesc_qk = make_idesc_f16(A3_BQ, A3_BK, BF16, false, false);
-      constexpr uint32_t idesc_pv = make_idesc_f16(A3_BQ, A3_D, BF16, false, true);   // V is MN-major
-      int kst = 0; uint32_t kph = 0;
-      int vst = 0; uint32_t vph = 0;
-      uint32_t qk_cnt = 0, pv_cnt = 0, item_cnt = 0;
-      const uint32_t p_addr = smem_u32(sP + t * A3_P);
-      const uint32_t s_tmem = tmem_base + t * A3_BK;
-      const uint32_t o_tmem = tmem_base + 256 + t * 64;
-      const uint32_t p_tmem = tmem_base + 384 + t * 64;
-      Attn3Items items(p, static_cast<int>(gridDim.x), static_cast<int>(blockIdx.x));
-      int qp_, head_, seq_;
-      bool b_active;
-      while (items.next(qp_, head_, seq_, b_active)) {
-        int j0_, j1_;
-        items.kv_range(n_kv, j0_, j1_);
-        const int n_it = j1_ - j0_;                          // kv tiles of this item (its split of the kv range)
-        if (!b_active && t == 1) {
-          // tile B has no rows in this item: only keep the shared K/V ring turning (its stages are released by
-          // BOTH tiles; waiting for `full` first keeps this thread from arriving twice in one phase)
-          for (int j = 0; j < n_it; ++j) {
-            mbar_wait(&k_full[kst], kph);
-            mbar_arrive(&k_empty[kst]);
-            if (++kst == A3_STAGES) { kst = 0; kph ^= 1; }
-            mbar_wait(&v_full[vst], vph);
-            mbar_arrive(&v_empty[vst]);
-            if (++vst == A3_STAGES) { vst = 0; vph ^= 1; }
-          }
-          continue;
-        }
-        const uint32_t qbuf = item_cnt & 1, qbpar = (item_cnt >> 1) & 1;   // item_cnt: items in which THIS tile took part
-        const uint32_t qpar = item_cnt & 1;
-        ++item_cnt;
-        const uint32_t q_addr = smem_u32(sQ + (qbuf * 2 + t) * A3_TILE);
-        mbar_wait(&q_full[qbuf * 2 + t], qbpar);
-        if (t == 1) mbar_wait(stagger, qpar);
-        for (int j = -1; j < n_it; ++j) {
-          // S(j+1): as soon as the softmax warps have pulled S(j) into registers
-          if (j + 1 < n_it) {
-            mbar_wait(&k_full[kst], kph);
-            mbar_wait(&s_empty[t], (qk_cnt & 1) ^ 1);
-            tc_fence_after();
-            const uint32_t k_addr = smem_u32(sK + kst * A3_TILE);
-#pragma unroll
-            for (int kk = 0; kk < A3_D / 16; ++kk)
-              umma_f16(s_tmem, make_desc_sw128(q_addr + kk * 32, 1024), make_desc_sw128(k_addr + kk * 32, 1024),
-                       idesc_qk, kk != 0 ? 1u : 0u);
-            umma_commit(&s_full[t]);
-            umma_commit(&k_empty[kst]);
-            ++qk_cnt;
-            if (++kst == A3_STAGES) { kst = 0; kph ^= 1; }
-          } else {
-            umma_commit(&q_empty[qbuf * 2 + t]);
-          }
-          if (j < 0) continue;
-          // O += P(j) V(j)
-          mbar_wait(&v_full[vst], vph);
-          mbar_wait(&p_full[t], pv_cnt & 1);
-          if (j == 0) mbar_wait(&o_free[t], qpar ^ 1);       // previous item's O has been read out
-          tc_fence_after();
-          const uint32_t v_addr = smem_u32(sV + vst * A3_TILE);
-#pragma unroll
-          for (int kk = 0; kk < A3_BK / 16; ++kk) {
-            if constexpr (PT)
-              umma_f16_ts(o_tmem, p_tmem + kk * 8, make_desc_sw128(v_addr + kk * 2048, 1024), idesc_pv,
-                          (j > 0 || kk != 0) ? 1u : 0u);
-            else
-              umma_f16(o_tmem, make_desc_sw128(p_addr + (kk >> 2) * 16384 + (kk & 3) * 32, 1024),
-                       make_desc_sw128(v_addr + kk * 2048, 1024), idesc_pv, (j > 0 || kk != 0) ? 1u : 0u);
-          }
-          umma_commit(&o_full[t]);
-          umma_commit(&p_empty[t]);
-          umma_commit(&v_empty[vst]);
-          ++pv_cnt;
-          if (++vst == A3_STAGES) { vst = 0; vph ^= 1; }
-        }
-      }
     }
   } else {
-    // -------------------------------------------------------------------- softmax warps (16)
-    asm volatile("setmaxnreg.inc.sync.aligned.u32 104;");
-    const int t = (warp - 4) >> 3;                 // query tile
-    const int h = ((warp - 4) >> 2) & 1;           // column half of the kv tile / of O
-    const int ew = warp & 3;                       // TMEM lane quarter
-    const int row = ew * 32 + lane;
-    const uint32_t lane_off = static_cast<uint32_t>(ew * 32) << 16;
-    const uint32_t tS = tmem_base + t * A3_BK + h * 64 + lane_off;
-    const uint32_t tO = tmem_base + 256 + t * 64 + h * 32 + lane_off;
-    const uint32_t tP = tmem_base + 384 + t * 64 + h * 32 + lane_off;
-    uint8_t* const pb = sP + t * A3_P + h * 16384 + row * 128;
-    float* const xm = xchg + (t * 2 + h) * 128 + row;          // my slot
-    float* const xo = xchg + (t * 2 + (1 - h)) * 128 + row;    // the other half's slot
-    const uint32_t bar_id = 1 + t;
+    // -------------------------------------------------------------------- consumers (one warpgroup per query tile)
+    const int t = (warp - 4) >> 2;                 // query tile
+    const int gtid = threadIdx.x & 127;
+    const int ew = (warp - 4) & 3;                 // warp inside the warpgroup: fragment rows [16 ew, 16 ew + 16) of a half
+    const int quad = lane & 3;
     const float c = p.scale_log2;
-    uint32_t kv_cnt = 0;
+    int kst = 0; uint32_t kph = 0;
+    int vst = 0; uint32_t vph = 0;
+    uint32_t item_cnt = 0;                         // items in which THIS tile took part
     Attn3Items items(p, static_cast<int>(gridDim.x), static_cast<int>(blockIdx.x));
     int qp, head, seq;
     bool b_active;
     while (items.next(qp, head, seq, b_active)) {
-      if (!b_active && t == 1) continue;                             // no rows for tile B in this item
       int j0, j1;
       items.kv_range(n_kv, j0, j1);
       const int split = items.split;
-      float m = -INFINITY, l = 0.f;
-      for (int j = j0; j < j1; ++j, ++kv_cnt) {
-        mbar_wait(&s_full[t], kv_cnt & 1);
-        tc_fence_after();
-        float s[64];
-        {
-          uint32_t r0[32], r1[32];
-          tmem_ld_32x32(tS, r0);
-          tmem_ld_32x32(tS + 32, r1);
-          tmem_ld_wait();
-#pragma unroll
-          for (int i = 0; i < 32; ++i) { s[i] = __uint_as_float(r0[i]); s[32 + i] = __uint_as_float(r1[i]); }
+      if (!b_active && t == 1) {
+        // tile B has no rows in this item: only keep the shared K/V ring turning
+        for (int j = j0; j < j1; ++j) {
+          mbar_wait(&k_full[kst], kph);
+          if (gtid == 0) mbar_arrive(&k_empty[kst]);
+          if (++kst == A3_STAGES) { kst = 0; kph ^= 1; }
+          mbar_wait(&v_full[vst], vph);
+          if (gtid == 0) mbar_arrive(&v_empty[vst]);
+          if (++vst == A3_STAGES) { vst = 0; vph ^= 1; }
         }
-        tc_fence_before();
-        mbar_arrive(&s_empty[t]);
-        const int valid = p.Lk - j * A3_BK - h * 64;   // keys of my half that exist
-        if (valid < 64) {                              // warp-uniform, only the ragged last kv tile
-          __syncwarp();                                // keeps this a real branch: if-converted it costs 54 predicated
-#pragma unroll                                         // instructions on EVERY tile (12 % of the softmax loop)
-          for (int i = 0; i < 64; ++i) if (i >= valid) s[i] = -INFINITY;
-        }
-        float mx0 = fmaxf(s[0], s[1]), mx1 = fmaxf(s[2], s[3]);
-#pragma unroll
-        for (int i = 4; i < 64; i += 4) {
-          mx0 = fmaxf(mx0, fmaxf(s[i], s[i + 1]));
-          mx1 = fmaxf(mx1, fmaxf(s[i + 2], s[i + 3]));
-        }
-        const float mloc = fmaxf(mx0, mx1);
-        // lazy rescale: refresh the running max only when some row of this tile outgrew it by 2^TAU
-        const bool need = !((mloc - m) * c <= A3_TAU);     // true for m = -inf (first tile) and NaN-safe
-        if (bar_red_or(bar_id, 256, need)) {
-          *xm = mloc;
-          named_bar_sync(bar_id, 256);
-          const float m_new = fmaxf(m, fmaxf(mloc, *xo));
-          if (j > j0) {
-            const float f = ex2_approx((m - m_new) * c);
-            mbar_wait(&o_full[t], (kv_cnt - 1) & 1);       // P(j-1) V(j-1) has landed
-            tc_fence_after();
-            uint32_t r[32];
-            tmem_ld_32x32(tO, r);
-            tmem_ld_wait();
-#pragma unroll
-            for (int i = 0; i < 32; i += 2) {
-              const float2 v = fmul2(make_float2(__uint_as_float(r[i]), __uint_as_float(r[i + 1])), make_float2(f, f));
-              r[i] = __float_as_uint(v.x); r[i + 1] = __float_as_uint(v.y);
-            }
-            tmem_st_32x32(tO, r);
-            tmem_st_wait();
-            tc_fence_before();
-            l *= f;
-          }
-          m = m_new;
-        }
-        const float mc = m * c;
-        // scale-and-shift and the row sums run as packed fp32 pairs (FFMA2 / FADD2): same IEEE results, half the
-        // issue slots -- the softmax warps are bound by issue slots and MUFU, not by the FMA pipe
-        float2 sum01 = make_float2(0.f, 0.f), sum23 = make_float2(0.f, 0.f);
-        const float2 c2 = make_float2(c, c), nmc2 = make_float2(-mc, -mc);
-        const bool sig = (t == 0 && j == j0);
-        if (sig && p.stagger_at == 0) mbar_arrive(stagger);
-#pragma unroll
-        for (int q4 = 0; q4 < 4; ++q4) {
-#pragma unroll
-          for (int i = q4 * 16; i < q4 * 16 + 16; i += 4) {
-            float2 a = ffma2(make_float2(s[i], s[i + 1]), c2, nmc2);
-            float2 b = ffma2(make_float2(s[i + 2], s[i + 3]), c2, nmc2);
-            if (emu_pair(i / 2, EMU8)) a = ex2_emulated2(a);
-            else { a.x = ex2_approx(a.x); a.y = ex2_approx(a.y); }
-            if (emu_pair(i / 2 + 1, EMU8)) b = ex2_emulated2(b);
-            else { b.x = ex2_approx(b.x); b.y = ex2_approx(b.y); }
-            s[i] = a.x; s[i + 1] = a.y; s[i + 2] = b.x; s[i + 3] = b.y;
-            sum01 = fadd2(sum01, a);
-            sum23 = fadd2(sum23, b);
-          }
-          if (sig && p.stagger_at == q4 + 1) mbar_arrive(stagger);   // lets tile B's pipeline start part-way
-        }
-        l += (sum01.x + sum01.y) + (sum23.x + sum23.y);
-        mbar_wait(&p_empty[t], (kv_cnt & 1) ^ 1);
-        if constexpr (PT) {
-          uint32_t pk[32];
-#pragma unroll
-          for (int i = 0; i < 32; ++i) pk[i] = pack16x2<BF16>(s[2 * i], s[2 * i + 1]);
-          tc_fence_after();
-          tmem_st_32x32(tP, pk);
-          tmem_st_wait();
-          tc_fence_before();
-        } else {
-#pragma unroll
-          for (int ch = 0; ch < 8; ++ch) {
-            uint4 u;
-            u.x = pack16x2<BF16>(s[ch * 8 + 0], s[ch * 8 + 1]);
-            u.y = pack16x2<BF16>(s[ch * 8 + 2], s[ch * 8 + 3]);
-            u.z = pack16x2<BF16>(s[ch * 8 + 4], s[ch * 8 + 5]);
-            u.w = pack16x2<BF16>(s[ch * 8 + 6], s[ch * 8 + 7]);
-            *reinterpret_cast<uint4*>(pb + ((ch ^ (row & 7)) << 4)) = u;
-          }
-          fence_proxy_async_smem();
-        }
-        mbar_arrive(&p_full[t]);
+        continue;
       }
-      // ---- epilogue of the item: O / l
-      mbar_wait(&o_full[t], (kv_cnt - 1) & 1);
-      tc_fence_after();
-      uint32_t r[32];
-      tmem_ld_32x32(tO, r);
-      tmem_ld_wait();
-      tc_fence_before();
-      mbar_arrive(&o_free[t]);
-      *xm = l;
-      named_bar_sync(bar_id, 256);
-      const float l_tot = l + *xo;
-      const float inv = 1.0f / l_tot;
-      named_bar_sync(bar_id, 256);                         // slots are reused by the next item's first tile
-      const int qrow = (qp * 2 + t) * A3_BQ + row;
-      if (p.kv_splits > 1) {
-        // partial result of this kv split: un-normalised O (relative to this split's running max m) + (m, l)
-        if (qrow < p.Lq) {
-          const int64_t grow = static_cast<int64_t>(split) * p.num_seq * p.Lq + static_cast<int64_t>(seq) * p.Lq + qrow;
-          float4* dst = reinterpret_cast<float4*>(p.ws_o + grow * (p.H * A3_D) + head * A3_D + h * 32);
+      const uint32_t qbuf = item_cnt & 1, qbpar = (item_cnt >> 1) & 1;
+      ++item_cnt;
+      const uint32_t q_addr = smem_u32(sQ + (qbuf * 2 + t) * A3_TILE);
+      mbar_wait(&q_full[qbuf * 2 + t], qbpar);
+      float o[2][32];
+      float m[2][2], l[2][2];                      // [half][row r / r + 8]: running max (raw score units), partial sum
 #pragma unroll
-          for (int ch = 0; ch < 8; ++ch)
-            dst[ch] = make_float4(__uint_as_float(r[ch * 4]), __uint_as_float(r[ch * 4 + 1]), __uint_as_float(r[ch * 4 + 2]),
-                                  __uint_as_float(r[ch * 4 + 3]));
-          if (h == 0) *reinterpret_cast<float2*>(p.ws_ml + (grow * p.H + head) * 2) = make_float2(m, l_tot);
+      for (int hh = 0; hh < 2; ++hh) {
+#pragma unroll
+        for (int i = 0; i < 32; ++i) o[hh][i] = 0.f;
+        m[hh][0] = m[hh][1] = -INFINITY;
+        l[hh][0] = l[hh][1] = 0.f;
+      }
+      for (int j = j0; j < j1; ++j) {
+        mbar_wait(&k_full[kst], kph);
+        const uint32_t k_addr = smem_u32(sK + kst * A3_TILE);
+        const uint32_t v_addr = smem_u32(sV + vst * A3_TILE);
+        const int valid = p.Lk - j * A3_BK;            // keys of this tile that exist
+#pragma unroll
+        for (int hh = 0; hh < 2; ++hh) {
+#pragma unroll 1
+          for (int kh = 0; kh < 2; ++kh) {
+            // ---- S = Q K^T  (64 query rows x 64 keys: rows [64 hh, +64) of the tile, keys [64 kh, +64) of the kv tile)
+            float s[32];
+            wgmma_fence();
+#pragma unroll
+            for (int kk = 0; kk < A3_D / 16; ++kk)
+              wgmma_m64n64k16_ss<BF16>(s, make_desc_sw128(q_addr + hh * (64 * 128) + kk * 32, 1024),
+                                       make_desc_sw128(k_addr + kh * (64 * 128) + kk * 32, 1024), kk != 0 ? 1u : 0u);
+            wgmma_commit();
+            wgmma_wait<0>();
+            reg_fence(s);
+            if (hh == 1 && kh == 1 && gtid == 0) {
+              mbar_arrive(&k_empty[kst]);
+              if (j == j1 - 1) mbar_arrive(&q_empty[qbuf * 2 + t]);     // last use of this item's Q
+            }
+            const int kvalid = valid - kh * 64;
+            if (kvalid < 64) {                             // only the ragged last kv tile
+#pragma unroll
+              for (int jj = 0; jj < 8; ++jj) {
+                const int col = 8 * jj + 2 * quad;
+                if (col >= kvalid) { s[4 * jj] = -INFINITY; s[4 * jj + 2] = -INFINITY; }
+                if (col + 1 >= kvalid) { s[4 * jj + 1] = -INFINITY; s[4 * jj + 3] = -INFINITY; }
+              }
+            }
+            // ---- online softmax (each row is spread over the 4 threads of a quad)
+            float mx0 = s[0], mx1 = s[2];
+#pragma unroll
+            for (int jj = 0; jj < 8; ++jj) {
+              mx0 = fmaxf(mx0, fmaxf(s[4 * jj], s[4 * jj + 1]));
+              mx1 = fmaxf(mx1, fmaxf(s[4 * jj + 2], s[4 * jj + 3]));
+            }
+            mx0 = fmaxf(mx0, __shfl_xor_sync(0xffffffffu, mx0, 1));
+            mx0 = fmaxf(mx0, __shfl_xor_sync(0xffffffffu, mx0, 2));
+            mx1 = fmaxf(mx1, __shfl_xor_sync(0xffffffffu, mx1, 1));
+            mx1 = fmaxf(mx1, __shfl_xor_sync(0xffffffffu, mx1, 2));
+            const float mn0 = fmaxf(m[hh][0], mx0), mn1 = fmaxf(m[hh][1], mx1);
+            if (j > j0 || kh > 0) {
+              // a fully masked slice leaves the running max in place (mn == m): f = 1
+              const float f0 = ex2_approx((m[hh][0] - mn0) * c), f1 = ex2_approx((m[hh][1] - mn1) * c);
+#pragma unroll
+              for (int jj = 0; jj < 8; ++jj) {
+                o[hh][4 * jj] *= f0; o[hh][4 * jj + 1] *= f0; o[hh][4 * jj + 2] *= f1; o[hh][4 * jj + 3] *= f1;
+              }
+              l[hh][0] *= f0; l[hh][1] *= f1;
+            }
+            m[hh][0] = mn0; m[hh][1] = mn1;
+            const float nmc0 = -mn0 * c, nmc1 = -mn1 * c;
+            uint32_t pa[4][4];                             // P as the A fragments of the 4 k16 steps of P V
+#pragma unroll
+            for (int kk = 0; kk < 4; ++kk) {
+              float e[8];
+#pragma unroll
+              for (int h = 0; h < 2; ++h) {
+                const int jj = 2 * kk + h;
+                e[4 * h + 0] = ex2_approx(fmaf(s[4 * jj], c, nmc0));
+                e[4 * h + 1] = ex2_approx(fmaf(s[4 * jj + 1], c, nmc0));
+                e[4 * h + 2] = ex2_approx(fmaf(s[4 * jj + 2], c, nmc1));
+                e[4 * h + 3] = ex2_approx(fmaf(s[4 * jj + 3], c, nmc1));
+              }
+              l[hh][0] += (e[0] + e[1]) + (e[4] + e[5]);
+              l[hh][1] += (e[2] + e[3]) + (e[6] + e[7]);
+              pa[kk][0] = pack16x2<BF16>(e[0], e[1]);      // row r,     keys 16 kk + 2 quad + {0, 1}
+              pa[kk][1] = pack16x2<BF16>(e[2], e[3]);      // row r + 8
+              pa[kk][2] = pack16x2<BF16>(e[4], e[5]);      // row r,     keys 16 kk + 8 + 2 quad + {0, 1}
+              pa[kk][3] = pack16x2<BF16>(e[6], e[7]);      // row r + 8
+            }
+            // ---- O += P V  (V rows [64 kh, +64) of the kv tile)
+            if (hh == 0 && kh == 0) mbar_wait(&v_full[vst], vph);
+            wgmma_fence();
+#pragma unroll
+            for (int kk = 0; kk < 4; ++kk)
+              wgmma_m64n64k16_rs_tb<BF16>(o[hh], pa[kk], make_desc_sw128(v_addr + kh * (64 * 128) + kk * 2048, 1024), 1u);
+            wgmma_commit();
+            wgmma_wait<0>();
+            reg_fence(o[hh]);
+          }
         }
-      } else if (qrow < p.Lq) {
-        uint16_t* dst = reinterpret_cast<uint16_t*>(p.o) + (static_cast<int64_t>(seq) * p.Lq + qrow) * p.ldo +
-                        head * A3_D + h * 32;
+        if (gtid == 0) mbar_arrive(&v_empty[vst]);
+        if (++kst == A3_STAGES) { kst = 0; kph ^= 1; }
+        if (++vst == A3_STAGES) { vst = 0; vph ^= 1; }
+      }
+      // ---- epilogue of the item
 #pragma unroll
-        for (int ch = 0; ch < 4; ++ch) {
-          uint4 u;
-          u.x = pack16x2<BF16>(__uint_as_float(r[ch * 8 + 0]) * inv, __uint_as_float(r[ch * 8 + 1]) * inv);
-          u.y = pack16x2<BF16>(__uint_as_float(r[ch * 8 + 2]) * inv, __uint_as_float(r[ch * 8 + 3]) * inv);
-          u.z = pack16x2<BF16>(__uint_as_float(r[ch * 8 + 4]) * inv, __uint_as_float(r[ch * 8 + 5]) * inv);
-          u.w = pack16x2<BF16>(__uint_as_float(r[ch * 8 + 6]) * inv, __uint_as_float(r[ch * 8 + 7]) * inv);
-          *reinterpret_cast<uint4*>(dst + ch * 8) = u;
+      for (int hh = 0; hh < 2; ++hh) {
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          float lt = l[hh][h];
+          lt += __shfl_xor_sync(0xffffffffu, lt, 1);
+          lt += __shfl_xor_sync(0xffffffffu, lt, 2);
+          const int qrow = (qp * 2 + t) * A3_BQ + hh * 64 + ew * 16 + (lane >> 2) + 8 * h;
+          if (qrow >= p.Lq) continue;
+          if (p.kv_splits > 1) {
+            // partial result of this kv split: un-normalised O (relative to this split's running max m) + (m, l)
+            const int64_t grow = static_cast<int64_t>(split) * p.num_seq * p.Lq + static_cast<int64_t>(seq) * p.Lq + qrow;
+            float* dst = p.ws_o + grow * (p.H * A3_D) + head * A3_D + 2 * quad;
+#pragma unroll
+            for (int jj = 0; jj < 8; ++jj)
+              *reinterpret_cast<float2*>(dst + 8 * jj) = make_float2(o[hh][4 * jj + 2 * h], o[hh][4 * jj + 2 * h + 1]);
+            if (quad == 0) *reinterpret_cast<float2*>(p.ws_ml + (grow * p.H + head) * 2) = make_float2(m[hh][h], lt);
+          } else {
+            const float inv = 1.0f / lt;
+            uint16_t* dst = reinterpret_cast<uint16_t*>(p.o) + (static_cast<int64_t>(seq) * p.Lq + qrow) * p.ldo +
+                            head * A3_D + 2 * quad;
+#pragma unroll
+            for (int jj = 0; jj < 8; ++jj)
+              *reinterpret_cast<uint32_t*>(dst + 8 * jj) =
+                  pack16x2<BF16>(o[hh][4 * jj + 2 * h] * inv, o[hh][4 * jj + 2 * h + 1] * inv);
+          }
         }
       }
     }
-  }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 2) {
-    tc_fence_after();
-    tmem_dealloc<512>(tmem_base);
   }
 }
 
@@ -576,10 +385,10 @@ attention3_merge_kernel(const float* __restrict__ ws_o, const float* __restrict_
   *dst = pack16x2<BF16>(acc.x * inv, acc.y * inv);
 }
 
-template <bool BF16, int EMU8, bool PT>
+template <bool BF16>
 int launch_attention3(const CUtensorMap& tQ, const CUtensorMap& tK, const CUtensorMap& tV, const Attn3Params& p,
                       cudaStream_t stream) {
-  auto kern = attention3_kernel<BF16, EMU8, PT>;
+  auto kern = attention3_kernel<BF16>;
   static DeviceOnce once;
   if (once.first()) {
     cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, A3_SMEM);
@@ -595,10 +404,10 @@ int launch_attention3(const CUtensorMap& tQ, const CUtensorMap& tK, const CUtens
 using namespace iggt;
 
 namespace {
-// Cost (in kv-tile steps of one CTA, ~1.4 us) of running the launch with `splits` kv ranges on `sms` CTAs: rounds x (tiles
-// per split + a fixed per-item overhead: Q load, pipeline fill, first-tile max, O read-out) + the merge pass over the fp32
-// workspace.  Constants fitted to the B200 sweep profiles/r02b_attn_sweep.json (1 of 8 / 4 / 2 views against 8 views of
-// keys, 1..5 splits): 7 steps per item, 8 steps + traffic for the merge launch; predictions within 6 % of measured.
+// Cost (in kv-tile steps of one CTA) of running the launch with `splits` kv ranges on `sms` CTAs: rounds x (tiles per
+// split + a fixed per-item overhead: Q load, pipeline fill, first-tile max, O read-out) + the merge pass over the fp32
+// workspace.  Model constants (estimates, not fitted on this kernel): 7 steps per item, 8 steps + workspace traffic for
+// the merge launch.
 double attn3_cost(int num_seq, int Lq, int Lk, int H, int splits, int sms) {
   const int q_tiles = (Lq + A3_BQ - 1) / A3_BQ, n_kv = (Lk + A3_BK - 1) / A3_BK;
   const int tps = (n_kv + splits - 1) / splits, se = (n_kv + tps - 1) / tps;
@@ -615,7 +424,7 @@ double attn3_cost(int num_seq, int Lq, int Lk, int H, int splits, int sms) {
   double cost = rounds * (tps + 7.0);
   if (se > 1) {
     const double ws_bytes = 2.0 * se * num_seq * Lq * H * A3_D * 4;     // written + read back
-    cost += 8.0 + ws_bytes / 8.0e12 / 1.4e-6;                            // workspace stays in L2; 1.4 us per kv-tile step
+    cost += 8.0 + ws_bytes / 8.0e12 / 1.4e-6;                            // workspace stays in L2 (model constants)
   }
   return cost;
 }
@@ -717,21 +526,7 @@ int attention_launch(const void* q, int64_t ldq, const void* k, int64_t ldk, con
   }
   p.ldo = ldo; p.o = o;
   p.scale_log2 = scale * 1.4426950408889634f;
-  static const int stag = [] { const char* e = getenv("IGGT_ATTN_STAG"); return e ? atoi(e) : 2; }();
-  p.stagger_at = stag < 0 ? 0 : (stag > 4 ? 4 : stag);
-  // IGGT_ATTN_EMU=1: 2 of every 8 probability pairs take the packed FMA-pipe exp2 (ex2_emulated2).  Measured on B200
-  // (profiles/r02b_attn_sweep.json: 0..4 of 8 pairs -> global 638 / 675 / 654 / 656 / 706 us, frame 124 / 128 / 124 /
-  // 124 / 132 us): no variant beats the MUFU-only kernel - halving the MUFU work makes the kernel SLOWER, so the softmax
-  // warps are bound by their dependency chain (S load -> max -> bar.red -> exp -> P store), not by MUFU throughput.
-  // Kept as an off-by-default experiment.  IGGT_ATTN_PT=0 keeps P in shared memory (the pre-TMEM variant).
-  static const int emu = [] { const char* e = getenv("IGGT_ATTN_EMU"); int v = e ? atoi(e) : A3_DEFAULT_EMU8; return v > 0 ? 2 : 0; }();
-  static const int pt = [] { const char* e = getenv("IGGT_ATTN_PT"); return e ? atoi(e) : 1; }();
-  int st;
-  if (!pt) st = dtype ? launch_attention3<true, 0, false>(tQ, tK, tV, p, s) : launch_attention3<false, 0, false>(tQ, tK, tV, p, s);
-  else switch (emu) {
-    case 2: st = dtype ? launch_attention3<true, 2, true>(tQ, tK, tV, p, s) : launch_attention3<false, 2, true>(tQ, tK, tV, p, s); break;
-    default: st = dtype ? launch_attention3<true, 0, true>(tQ, tK, tV, p, s) : launch_attention3<false, 0, true>(tQ, tK, tV, p, s);
-  }
+  const int st = dtype ? launch_attention3<true>(tQ, tK, tV, p, s) : launch_attention3<false>(tQ, tK, tV, p, s);
   if (st != 0 || p.kv_splits == 1) return st;
   const int64_t warps = rows * H;
   const unsigned grid = static_cast<unsigned>((warps + 7) / 8);

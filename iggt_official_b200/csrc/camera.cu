@@ -1,10 +1,9 @@
 // The whole camera head (iggt/heads/camera_head.py:83-154 + head_act.py:12-35) as ONE persistent kernel.
 //
 // M = B*S <= 16 camera tokens against 216 M parameters, four refinement iterations: every Linear is a weight stream
-// (1.7 GB of 16-bit weights per forward, 0.27 ms at HBM speed) with a few MFLOP of work, but as separate launches it is
-// ~180 dependent kernels of 5-20 us each (LayerNorm / skinny GEMM / tiny attention / AdaLN glue), i.e. launch- and
-// latency-bound: 2.0 ms of the 54 ms C2 step on one GPU and 12 % of the step on each of 8 view-sharded ranks, where the
-// head is replicated.  Here the ~27 phases of an iteration run inside one grid of <= 128 CTAs with a device-wide barrier
+// (1.7 GB of 16-bit weights per forward, 0.5 ms at the H100's 3.35 TB/s) with a few MFLOP of work, but as separate
+// launches it is ~180 small dependent kernels (LayerNorm / skinny GEMM / tiny attention / AdaLN glue), i.e. launch- and
+// latency-bound, and on view-sharded ranks the head is replicated.  Here the ~27 phases of an iteration run inside one grid of <= 128 CTAs with a device-wide barrier
 // between phases:
 //   * warp 8 is a TMA producer that walks the same phase program AHEAD of the consumers: weight stages (ONE 3-D box
 //     {64 k, 16 columns, 16 k groups} = 1024 k x 16 columns = 32 KB per instruction, 128B-swizzled) of the next phases
@@ -16,9 +15,6 @@
 //   * the products run on the tensor cores (mma.sync.m16n8k16, fp32 accumulate): C[16 x 16] += (X_hi + X_lo) W^T, warp w
 //     takes every 8th k step of a stage, fragments come straight from the swizzled stage / the padded planes (bank-conflict
 //     free), the 8 warps' partial tiles meet in an 8 KB shared-memory reduction and thread (row, column) finishes one output.
-//     History (timelines under profiles/r02*_camera_*): three CUDA-core thread mappings all sat at 1.6-1.8 TB/s of weight
-//     streaming - the fp32 pipe (FFMA2 at one per 4 clk per scheduler) was the limit, and with the arithmetic removed the
-//     stream itself topped out at 3.0 TB/s because one thread issued one 8 KB TMA box at a time;
 //   * bias, exact-erf GELU / SiLU, LayerScale, residual and the pose accumulation + activation ride in the epilogue;
 //   * the S x S attention (16 heads x 128) is a phase of its own: one warp per (row, head).
 // fp32 accumulation, 16-bit weights, activations to ~2^-22 (fp16 weights) / 2^-16 (bf16) relative - within rounding of the

@@ -2,7 +2,7 @@
 #include <cuda_runtime.h>
 #include "../../include/iggt_b200.h"
 
-extern "C" const char* iggt_version(void) { return "iggt_b200 0.1 (sm_100a)"; }
+extern "C" const char* iggt_version(void) { return "iggt_b200 0.2 (sm_90a)"; }
 
 extern "C" int iggt_device_info(int* sm, int* num_sms) {
   int dev = 0;

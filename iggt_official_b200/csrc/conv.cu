@@ -1,4 +1,4 @@
-// C-ABI launcher: NHWC implicit-GEMM convolution (3x3 pad 1 / 1x1) on the tcgen05 GEMM main loop.
+// C-ABI launcher: NHWC implicit-GEMM convolution (3x3 pad 1 / 1x1) on the wgmma GEMM main loop.
 // The A operand of tap (ky,kx) is the 4-D TMA box {64 ch, 16 px, 8 rows, 1 image} shifted by
 // (kx-1, ky-1); TMA zero-fills the halo, so no im2col buffer is ever materialised.
 #include "gemm_launch.cuh"
@@ -8,14 +8,10 @@ using namespace iggt;
 
 namespace {
 template <bool BF16>
-int dispatch_bn(int bn, bool pair, const CUtensorMap& tA, const CUtensorMap& tB, const CUtensorMap& tC,
-                const GemmParams& p, cudaStream_t s) {
-  if (pair) return launch_gemm_kernel<256, EPI_STORE16, BF16, true, true>(tA, tB, tC, p, s);
-  switch (bn) {
-    case 256: return launch_gemm_kernel<256, EPI_STORE16, BF16, true>(tA, tB, tC, p, s);
-    case 128: return launch_gemm_kernel<128, EPI_STORE16, BF16, true>(tA, tB, tC, p, s);
-    default: return launch_gemm_kernel<64, EPI_STORE16, BF16, true>(tA, tB, tC, p, s);
-  }
+int dispatch_bn(int bn, const CUtensorMap& tA, const CUtensorMap& tB, const CUtensorMap& tC, const GemmParams& p,
+                cudaStream_t s) {
+  if (bn == 64) return launch_gemm_kernel<64, EPI_STORE16, BF16, true>(tA, tB, tC, p, s);
+  return launch_gemm_kernel<128, EPI_STORE16, BF16, true>(tA, tB, tC, p, s);
 }
 }  // namespace
 
@@ -35,8 +31,6 @@ extern "C" int iggt_conv_nhwc(const void* x, const void* Wp, void* out, int NB, 
   p.M = NB * H * W; p.N = Cout; p.K = taps * Cin;
   p.num_m_tiles = NB * p.tiles_x * p.tiles_y;
   const int bn = choose_bn(p.num_m_tiles, Cout);
-  const bool pair = use_pair(PAIR_CONV, bn, p.num_m_tiles);
-  if (pair) p.num_m_tiles = (p.num_m_tiles + 1) / 2;   // pairs of spatial tiles (gemm.cuh, PAIR)
   p.num_n_tiles = (Cout + bn - 1) / bn;
   p.num_k_blocks = taps * (Cin / GEMM_BK);
   p.add_rows = 1;
@@ -48,13 +42,13 @@ extern "C" int iggt_conv_nhwc(const void* x, const void* Wp, void* out, int NB, 
     uint32_t box[4] = {64, CONV_TW, CONV_TH, 1};
     if (make_tmap(&tA, dt, 4, x, dims, str, box)) return -4;
   }
-  if (make_tmap_2d(&tB, dt, Wp, Cout, (uint64_t)taps * Cin, (uint64_t)taps * Cin, GEMM_BK, pair ? bn / 2 : bn)) return -4;
+  if (make_tmap_2d(&tB, dt, Wp, Cout, (uint64_t)taps * Cin, (uint64_t)taps * Cin, GEMM_BK, bn)) return -4;
   {
     uint64_t dims[4] = {(uint64_t)Cout, (uint64_t)W, (uint64_t)H, (uint64_t)NB};
     uint64_t str[3] = {(uint64_t)Cout * 2, (uint64_t)W * Cout * 2, (uint64_t)H * W * Cout * 2};
     uint32_t box[4] = {64, CONV_TW, CONV_TH, 1};
     if (make_tmap(&tC, dt, 4, out, dims, str, box)) return -4;
   }
-  return dtype ? dispatch_bn<true>(bn, pair, tA, tB, tC, p, (cudaStream_t)stream)
-               : dispatch_bn<false>(bn, pair, tA, tB, tC, p, (cudaStream_t)stream);
+  return dtype ? dispatch_bn<true>(bn, tA, tB, tC, p, (cudaStream_t)stream)
+               : dispatch_bn<false>(bn, tA, tB, tC, p, (cudaStream_t)stream);
 }

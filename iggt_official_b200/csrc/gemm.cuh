@@ -1,12 +1,13 @@
-// Persistent, warp-specialised tcgen05 GEMM / implicit-GEMM convolution for sm_100a.
+// Persistent, warp-specialised wgmma GEMM / implicit-GEMM convolution for sm_90a.
 //
-//   D[M,N] = epilogue( A[M,K] (16-bit, K-major) x W[N,K]^T (16-bit, K-major), fp32 accumulate in TMEM )
+//   D[M,N] = epilogue( A[M,K] (16-bit, K-major) x W[N,K]^T (16-bit, K-major), fp32 accumulate in registers )
 //
-// One CTA per SM loops over 128 x BN output tiles (or, PAIR, two CTAs of a cluster over 256 x BN tiles with one
-// cta_group::2 MMA). Warp roles: warp 0 = TMA producer, warp 1 = MMA issuer (one elected thread), warp 2 = TMEM
-// allocator, warps 4.. = one or two 4-warp epilogue groups (TMEM -> registers -> swizzled smem staging -> TMA store /
-// TMA reduce-add). Two TMEM accumulator stages let the epilogue of tile i overlap the main loop of tile i+1; work is
-// handed out by WorkIter (whole tiles round-robin, or stream-K ranges of k-blocks for the residual epilogue).
+// One CTA per SM loops over 128 x BN output tiles (BN = 64 or 128). Warp roles: warp 0 = TMA producer (a ring of
+// 128B-swizzled A / W stages), warpgroups 1 and 2 = consumers: each issues the wgmma of 64 rows of the tile, then both
+// spill the fp32 accumulator to a shared-memory tile and act as two 4-warp epilogue groups (one row per thread,
+// 64-column chunks alternating between the groups: registers -> swizzled smem staging -> TMA store / TMA reduce-add).
+// The producer runs ahead into the next tile while the consumers work through an epilogue. Work is handed out by
+// WorkIter (whole tiles round-robin, or stream-K ranges of k-blocks for the residual epilogue).
 //
 // Reference call sites this replaces (all via torch.nn on the reference side, SURVEY.md §2.2):
 //   qkv   iggt/layers/attention.py:52-58   (+ q/k LayerNorm(64) and 2-D RoPE, rope.py:154-188)
@@ -76,22 +77,21 @@ struct GemmParams {
 
 constexpr int GEMM_BM = 128;
 constexpr int GEMM_BK = 64;
-constexpr int GEMM_THREADS = 256;
+constexpr int GEMM_THREADS = 384;
 constexpr int CONV_TW = 16;
 constexpr int CONV_TH = 8;
 
-// PAIR: the CTA is one half of a cta_group::2 pair working on a 256 x BN tile; it stages its own 128 rows of A and
-// HALF of the B tile (BN/2 weight rows) per k-block, so the per-SM smem fill drops from 48 KB to 32 KB per k-block
-// at BN = 256 (the 1-CTA kernel is bound by exactly that traffic: 97 B/clk of TMA writes + 96 B/clk of MMA reads).
-template <int BN, bool PAIR = false>
+template <int BN>
 struct GemmSmem {
   static constexpr int A_BYTES = GEMM_BM * GEMM_BK * 2;   // 16 KB
-  static constexpr int B_BYTES = (PAIR ? BN / 2 : BN) * GEMM_BK * 2;
+  static constexpr int B_BYTES = BN * GEMM_BK * 2;
   static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
   static constexpr int STG_BYTES = 16384;                 // 128 rows x 128 B staging tile
-  static constexpr int STAGES = PAIR ? (BN == 256 ? 6 : 8) : ((BN == 256) ? 4 : ((BN == 128) ? 6 : 8));
+  static constexpr int ACC_LD = BN + 8;                   // fp32 accumulator tile row pitch (conflict-free fragment stores)
+  static constexpr int ACC_BYTES = GEMM_BM * ACC_LD * 4;
+  static constexpr int STAGES = BN == 128 ? 3 : 6;
   static constexpr int VEC_BYTES = BN * 4 + (BN * 4 > 1024 ? BN * 4 : 1024);   // bias[BN] + (gamma[BN] | q/k-norm vectors [4][64])
-  static constexpr int TOTAL = STAGES * STAGE_BYTES + 2 * STG_BYTES + 256 /*barriers*/ + VEC_BYTES;
+  static constexpr int TOTAL = STAGES * STAGE_BYTES + ACC_BYTES + 2 * STG_BYTES + 256 /*barriers*/ + VEC_BYTES;
 };
 
 template <bool BF16>
@@ -150,36 +150,28 @@ struct WorkIter {
 };
 
 // CONV: A operand comes from a 4-D NHWC tensor map (box {64, TW, TH, 1}); otherwise 2-D [M,K].
-// G = epilogue warpgroups (1 or 2). With G = 2 the column chunks of a tile alternate between two 4-warp
-// groups (each TMEM lane quarter is then read by two warps), doubling epilogue issue slots and halving
-// the registers available per thread (384 threads) -- used for every epilogue except the qkv one.
-// PAIR = cta_group::2: launched as clusters of two CTAs; p.num_m_tiles then counts 256-row tile pairs and CTA `rank`
-// of the pair owns the 128-row sub-tile 2 * mt + rank (a sub-tile past the end of the problem is all TMA zero fill
-// on the way in and clipped on the way out).
-template <int BN, int EPI, bool BF16, bool CONV, int G, bool PAIR>
-__global__ void __launch_bounds__(128 + 128 * G, 1)
-gemm_tcgen05_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
-                    const __grid_constant__ CUtensorMap tmC, const GemmParams p) {
-  using SM = GemmSmem<BN, PAIR>;
+template <int BN, int EPI, bool BF16, bool CONV>
+__global__ void __launch_bounds__(GEMM_THREADS, 1)
+gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
+                  const __grid_constant__ CUtensorMap tmC, const GemmParams p) {
+  using SM = GemmSmem<BN>;
   constexpr int STAGES = SM::STAGES;
+  constexpr int G = 2;                                 // epilogue groups = consumer warpgroups
   extern __shared__ __align__(1024) uint8_t smem[];   // 128B-swizzled tiles need 1024-byte alignment
   if ((smem_u32(smem) & 1023u) != 0) __trap();
   uint8_t* smem_a = smem;
   uint8_t* smem_b = smem + STAGES * SM::A_BYTES;
-  uint8_t* staging = smem + STAGES * SM::STAGE_BYTES;
+  float* acc_tile = reinterpret_cast<float*>(smem + STAGES * SM::STAGE_BYTES);
+  uint8_t* staging = smem + STAGES * SM::STAGE_BYTES + SM::ACC_BYTES;
   uint64_t* bars = reinterpret_cast<uint64_t*>(staging + 2 * SM::STG_BYTES);
   uint64_t* full_bar = bars;
   uint64_t* empty_bar = bars + STAGES;
-  uint64_t* tfull_bar = bars + 2 * STAGES;
-  uint64_t* tempty_bar = bars + 2 * STAGES + 2;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 2 * STAGES + 4);
   float* epi_vec = reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(bars) + 256);
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
-  const uint32_t rank = PAIR ? cluster_ctarank() : 0u;          // 0 = the CTA that issues the pair's MMAs
-  const int worker = PAIR ? static_cast<int>(blockIdx.x >> 1) : static_cast<int>(blockIdx.x);
-  const int workers = PAIR ? static_cast<int>(gridDim.x >> 1) : static_cast<int>(gridDim.x);
+  const int worker = static_cast<int>(blockIdx.x);
+  const int workers = static_cast<int>(gridDim.x);
 
   if (warp == 0 && lane == 0) {
     tma_prefetch_desc(&tmA);
@@ -189,35 +181,23 @@ gemm_tcgen05_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_consta
   if (warp == 1 && lane == 0) {
     for (int i = 0; i < STAGES; ++i) {
       mbar_init(&full_bar[i], 1);
-      mbar_init(&empty_bar[i], 1);
-    }
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(&tfull_bar[i], 1);
-      mbar_init(&tempty_bar[i], 4 * G * (PAIR ? 2 : 1));   // PAIR: the epilogue warps of both CTAs release rank 0's
+      mbar_init(&empty_bar[i], G);                     // one arrival per consumer warpgroup
     }
     fence_barrier_init();
   }
-  if (warp == 2) {
-    if constexpr (PAIR) tmem_alloc_pair<2 * BN>(tmem_slot);
-    else tmem_alloc<2 * BN>(tmem_slot);
-  }
-  tc_fence_before();
-  if constexpr (PAIR) cluster_sync_all();   // the peer's barriers must be initialised before anything signals them
-  else __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
+  __syncthreads();
   griddep_wait();      // PDL: everything above overlapped the previous kernel's tail
   griddep_launch();
 
-  if (warp == 0) {
+  if (warp < 4) {
     // ------------------------------------------------------------ TMA producer
-    if (lane == 0) {
+    if (warp == 0 && lane == 0) {
       int stage = 0;
       uint32_t phase = 0;
       WorkIter work(p, worker, workers);
       int tile, kb0, kb1;
       while (work.next(tile, kb0, kb1)) {
-        const int mt = (tile / p.num_n_tiles) * (PAIR ? 2 : 1) + static_cast<int>(rank);
+        const int mt = tile / p.num_n_tiles;
         const int nt = tile % p.num_n_tiles;
         int img = 0, y0 = 0, x0 = 0;
         if constexpr (CONV) {
@@ -236,72 +216,25 @@ gemm_tcgen05_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_consta
             c0 = (kb % cblocks) * GEMM_BK;
             if (p.conv_taps == 9) { dy = tap / 3 - 1; dx = tap % 3 - 1; }
           }
-          if constexpr (PAIR) {
-            // both CTAs' bytes are credited to rank 0's barrier; rank 0 posts the expectation for the pair
-            if (rank == 0) mbar_expect_tx(&full_bar[stage], 2 * SM::STAGE_BYTES);
-            const uint32_t fb = mapa_u32(&full_bar[stage], 0);
-            if constexpr (CONV) tma_load_4d_pair(smem_a + stage * SM::A_BYTES, &tmA, fb, c0, x0 + dx, y0 + dy, img);
-            else tma_load_2d_pair(smem_a + stage * SM::A_BYTES, &tmA, fb, kb * GEMM_BK, mt * GEMM_BM);
-            tma_load_2d_pair(smem_b + stage * SM::B_BYTES, &tmB, fb, kb * GEMM_BK,
-                             nt * BN + static_cast<int>(rank) * (BN / 2));
-          } else {
-            mbar_expect_tx(&full_bar[stage], SM::STAGE_BYTES);
-            if constexpr (CONV) tma_load_4d(smem_a + stage * SM::A_BYTES, &tmA, &full_bar[stage], c0, x0 + dx, y0 + dy, img);
-            else tma_load_2d(smem_a + stage * SM::A_BYTES, &tmA, &full_bar[stage], kb * GEMM_BK, mt * GEMM_BM);
-            tma_load_2d(smem_b + stage * SM::B_BYTES, &tmB, &full_bar[stage], kb * GEMM_BK, nt * BN);
-          }
+          mbar_expect_tx(&full_bar[stage], SM::STAGE_BYTES);
+          if constexpr (CONV) tma_load_4d(smem_a + stage * SM::A_BYTES, &tmA, &full_bar[stage], c0, x0 + dx, y0 + dy, img);
+          else tma_load_2d(smem_a + stage * SM::A_BYTES, &tmA, &full_bar[stage], kb * GEMM_BK, mt * GEMM_BM);
+          tma_load_2d(smem_b + stage * SM::B_BYTES, &tmB, &full_bar[stage], kb * GEMM_BK, nt * BN);
           if (++stage == STAGES) { stage = 0; phase ^= 1; }
         }
       }
     }
-  } else if (warp == 1) {
-    // ------------------------------------------------------------ MMA issuer
-    if (lane == 0 && rank == 0) {
-      constexpr uint32_t idesc = make_idesc_f16(PAIR ? 2 * GEMM_BM : GEMM_BM, BN, BF16, false, false);
-      int stage = 0;
-      uint32_t phase = 0;
-      int acc = 0;
-      uint32_t acc_phase = 0;
-      WorkIter work(p, worker, workers);
-      int tile, kb0, kb1;
-      while (work.next(tile, kb0, kb1)) {
-        mbar_wait(&tempty_bar[acc], acc_phase ^ 1);
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + acc * BN;
-        for (int kb = kb0; kb < kb1; ++kb) {
-          mbar_wait(&full_bar[stage], phase);
-          tc_fence_after();
-          const uint32_t a_addr = smem_u32(smem_a + stage * SM::A_BYTES);
-          const uint32_t b_addr = smem_u32(smem_b + stage * SM::B_BYTES);
-#pragma unroll
-          for (int k = 0; k < GEMM_BK / 16; ++k) {
-            const uint64_t da = make_desc_sw128(a_addr + k * 32, 1024);
-            const uint64_t db = make_desc_sw128(b_addr + k * 32, 1024);
-            if constexpr (PAIR) umma_f16_pair(d_tmem, da, db, idesc, (kb != kb0 || k != 0) ? 1u : 0u);
-            else umma_f16(d_tmem, da, db, idesc, (kb != kb0 || k != 0) ? 1u : 0u);
-          }
-          // frees the smem slot (of both CTAs) when these MMAs retire
-          if constexpr (PAIR) umma_commit_pair(&empty_bar[stage]);
-          else umma_commit(&empty_bar[stage]);
-          if (++stage == STAGES) { stage = 0; phase ^= 1; }
-        }
-        // accumulator complete -> epilogue (of both CTAs)
-        if constexpr (PAIR) umma_commit_pair(&tfull_bar[acc]);
-        else umma_commit(&tfull_bar[acc]);
-        if (++acc == 2) { acc = 0; acc_phase ^= 1; }
-      }
-    }
-  } else if (warp >= 4) {
-    // ------------------------------------------------------------ epilogue (128 threads, 1 row each)
-    const int grp = (warp - 4) >> 2;       // epilogue group
-    const int ew = (warp - 4) & 3;         // == warp % 4 -> TMEM lanes [32*ew, 32*ew+32)
-    const int row = ew * 32 + lane;        // row inside the tile
+  } else {
+    // ------------------------------------------------------------ consumers: main loop, then epilogue (1 row / thread)
+    const int grp = (warp - 4) >> 2;       // consumer warpgroup = epilogue group
+    const int ew = (warp - 4) & 3;         // warp inside the group
+    const int row = ew * 32 + lane;        // epilogue: row inside the tile
     const bool leader = (ew == 0 && lane == 0);
     constexpr int NBUF = 2 / G;            // staging buffers per group
     uint8_t* const stg_grp = staging + grp * NBUF * SM::STG_BYTES;
     const uint32_t bar_id = 1 + grp;
     const int gtid = ew * 32 + lane;       // thread index inside the group
-    float* const vb = epi_vec;                  // this tile's bias   [BN]  (staged before the accumulator is ready)
+    float* const vb = epi_vec;                  // this tile's bias   [BN]
     float* const vg = vb + BN;                  // this tile's gamma  [BN]  (EPI_RESID32)
     float* const vn = vb + BN;                  // q_norm w,b | k_norm w,b  [4][64]  (EPI_QKV, BN >= 128)
     if constexpr (epi_is_qkv(EPI)) {
@@ -311,20 +244,43 @@ gemm_tcgen05_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_consta
         }
       }
     }
-    int acc = 0;
-    uint32_t acc_phase = 0;
+    int stage = 0;
+    uint32_t phase = 0;
     uint32_t store_count = 0;
     WorkIter work(p, worker, workers);
     int tile, kb0, kb1;
-    // releasing an accumulator stage: one arrival per epilogue warp on the MMA issuer's (rank 0's) barrier
-    auto release_acc = [&](int a) {
-      if constexpr (PAIR) mbar_arrive_cluster(mapa_u32(&tempty_bar[a], 0));
-      else mbar_arrive(&tempty_bar[a]);
-    };
     while (work.next(tile, kb0, kb1)) {
-      const int mt = (tile / p.num_n_tiles) * (PAIR ? 2 : 1) + static_cast<int>(rank);
+      const int mt = tile / p.num_n_tiles;
       const int nt = tile % p.num_n_tiles;
       const int n0 = nt * BN;
+      // ---- main loop: rows [64 grp, 64 grp + 64) of the tile
+      float acc[BN / 2];
+#pragma unroll
+      for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+      int prev_stage = -1;
+      for (int kb = kb0; kb < kb1; ++kb) {
+        mbar_wait(&full_bar[stage], phase);
+        const uint32_t a_addr = smem_u32(smem_a + stage * SM::A_BYTES) + grp * (64 * 128);
+        const uint32_t b_addr = smem_u32(smem_b + stage * SM::B_BYTES);
+        wgmma_fence();
+#pragma unroll
+        for (int k = 0; k < GEMM_BK / 16; ++k) {
+          const uint64_t da = make_desc_sw128(a_addr + k * 32, 1024);
+          const uint64_t db = make_desc_sw128(b_addr + k * 32, 1024);
+          if constexpr (BN == 128) wgmma_m64n128k16_ss<BF16>(acc, da, db, (kb != kb0 || k != 0) ? 1u : 0u);
+          else wgmma_m64n64k16_ss<BF16>(acc, da, db, (kb != kb0 || k != 0) ? 1u : 0u);
+        }
+        wgmma_commit();
+        // the previous k-block's MMAs have retired once at most this one is pending: free its smem slot
+        wgmma_wait<1>();
+        if (prev_stage >= 0 && gtid == 0) mbar_arrive(&empty_bar[prev_stage]);
+        prev_stage = stage;
+        if (++stage == STAGES) { stage = 0; phase ^= 1; }
+      }
+      wgmma_wait<0>();
+      reg_fence(acc);
+      if (prev_stage >= 0 && gtid == 0) mbar_arrive(&empty_bar[prev_stage]);
+
       int img = 0, y0 = 0, x0 = 0;
       long grow;                           // global row (pixel) index of this thread, -1 if out of range
       if constexpr (CONV) {
@@ -339,26 +295,27 @@ gemm_tcgen05_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_consta
         grow = (long)mt * GEMM_BM + row;
         if (grow >= p.M) grow = -1;
       }
-      // stage the tile's per-column vectors in smem while the MMAs of this tile are still running
-      // (with the smem carve-out this kernel uses there is no L1 left to cache them)
-      named_bar_sync(3, 128 * G);          // every epilogue thread is done with the previous tile's vectors
+      // ---- accumulator fragments -> fp32 tile in smem (one row per epilogue thread from here on), per-column vectors
+      named_bar_sync(3, 128 * G);          // every epilogue thread is done with the previous tile's accumulator / vectors
+      {
+        const int r0 = grp * 64 + ew * 16 + (lane >> 2);
+        float* const d0 = acc_tile + r0 * SM::ACC_LD + 2 * (lane & 3);
+#pragma unroll
+        for (int j = 0; j < BN / 8; ++j) {
+          *reinterpret_cast<float2*>(d0 + 8 * j) = make_float2(acc[4 * j], acc[4 * j + 1]);
+          *reinterpret_cast<float2*>(d0 + 8 * SM::ACC_LD + 8 * j) = make_float2(acc[4 * j + 2], acc[4 * j + 3]);
+        }
+      }
       for (int i = grp * 128 + gtid; i < BN; i += 128 * G) {
         const int col = n0 + i;
         vb[i] = (p.bias && col < p.N && kb0 == 0) ? __ldg(p.bias + col) : 0.f;   // bias rides with the first K segment
         if constexpr (EPI == EPI_RESID32) vg[i] = (p.gamma && col < p.N) ? __ldg(p.gamma + col) : 1.f;
       }
       named_bar_sync(3, 128 * G);
-      mbar_wait(&tfull_bar[acc], acc_phase);
-      tc_fence_after();
-      const uint32_t t_row = tmem_base + (static_cast<uint32_t>(ew * 32) << 16) + acc * BN;
+      const float* const t_row = acc_tile + row * SM::ACC_LD;
 
       if constexpr (EPI == EPI_STORE16 || epi_is_qkv(EPI)) {
         const int nvalid = min(BN / 64, (p.N - n0 + 63) / 64);
-        if (grp >= nvalid) {               // nothing to read for this group: release immediately
-          tc_fence_before();
-          __syncwarp();
-          if (lane == 0) release_acc(acc);
-        }
 #pragma unroll 1
         for (int c64 = grp; c64 < nvalid; c64 += G) {
           const int col0 = n0 + c64 * 64;
@@ -366,19 +323,10 @@ gemm_tcgen05_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_consta
           if (leader) tma_store_wait_read<NBUF - 1>();
           named_bar_sync(bar_id, 128);
           float v[64];
-          {
-            uint32_t r0[32], r1[32];
-            tmem_ld_32x32(t_row + c64 * 64, r0);
-            tmem_ld_32x32(t_row + c64 * 64 + 32, r1);
-            tmem_ld_wait();
 #pragma unroll
-            for (int i = 0; i < 32; ++i) { v[i] = __uint_as_float(r0[i]); v[32 + i] = __uint_as_float(r1[i]); }
-          }
-          if (c64 + G >= nvalid) {
-            // last TMEM read of this tile by this warp: release the accumulator stage
-            tc_fence_before();
-            __syncwarp();
-            if (lane == 0) release_acc(acc);
+          for (int i = 0; i < 64; i += 4) {
+            const float4 a = *reinterpret_cast<const float4*>(t_row + c64 * 64 + i);
+            v[i] = a.x; v[i + 1] = a.y; v[i + 2] = a.z; v[i + 3] = a.w;
           }
           {
 #pragma unroll
@@ -530,28 +478,18 @@ gemm_tcgen05_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_consta
       } else {
         // fp32 outputs: 32 columns (128 B) per staging tile
         const int nvalid = min(BN / 32, (p.N - n0 + 31) / 32);
-        if (grp >= nvalid) {
-          tc_fence_before();
-          __syncwarp();
-          if (lane == 0) release_acc(acc);
-        }
 #pragma unroll 1
         for (int c32 = grp; c32 < nvalid; c32 += G) {
           const int col0 = n0 + c32 * 32;
           uint8_t* stg = stg_grp + (store_count % NBUF) * SM::STG_BYTES;
           if (leader) tma_store_wait_read<NBUF - 1>();
           named_bar_sync(bar_id, 128);
-          uint32_t r0[32];
-          tmem_ld_32x32(t_row + c32 * 32, r0);
-          tmem_ld_wait();
-          if (c32 + G >= nvalid) {
-            tc_fence_before();
-            __syncwarp();
-            if (lane == 0) release_acc(acc);
-          }
           float v[32];
 #pragma unroll
-          for (int i = 0; i < 32; ++i) v[i] = __uint_as_float(r0[i]);
+          for (int i = 0; i < 32; i += 4) {
+            const float4 a = *reinterpret_cast<const float4*>(t_row + c32 * 32 + i);
+            v[i] = a.x; v[i + 1] = a.y; v[i + 2] = a.z; v[i + 3] = a.w;
+          }
 #pragma unroll
           for (int i = 0; i < 32; i += 4) {
             const float4 b = *reinterpret_cast<const float4*>(vb + c32 * 32 + i);
@@ -589,7 +527,6 @@ gemm_tcgen05_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_consta
           ++store_count;
         }
       }
-      if (++acc == 2) { acc = 0; acc_phase ^= 1; }
     }
     if (leader) {
       tma_store_wait_all<0>();
@@ -597,15 +534,6 @@ gemm_tcgen05_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_consta
         if (p.n_gather > 0) __threadfence_system();      // peer stores visible before the cross-rank barrier
       }
     }
-  }
-
-  tc_fence_before();
-  if constexpr (PAIR) cluster_sync_all();   // neither CTA may exit (or free TMEM) while its peer can still touch it
-  else __syncthreads();
-  if (warp == 2) {
-    tc_fence_after();
-    if constexpr (PAIR) tmem_dealloc_pair<2 * BN>(tmem_base);
-    else tmem_dealloc<2 * BN>(tmem_base);
   }
 }
 

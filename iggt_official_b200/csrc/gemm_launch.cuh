@@ -5,35 +5,15 @@
 
 namespace iggt {
 
-// Pick the N tile: fewest "wave-quantised" tile-slots; ties go to the wider tile (less smem traffic
-// per MAC: a 128x256 tile reads 96 B/clk of operands, 128x128 reads 128 B/clk).
-inline int choose_bn(int m_tiles, int N) {
-  if (N <= 64) return 64;
-  if (N <= 128) return 128;
-  const int sms = device_sm_count();
-  auto cost = [&](int bn) {
-    long tiles = (long)m_tiles * ((N + bn - 1) / bn);
-    long waves = (tiles + sms - 1) / sms;
-    return waves * bn;  // time ~ waves x tile width
-  };
-  long c256 = cost(256), c128 = cost(128);
-  return (c128 * 100 < c256 * 92) ? 128 : 256;
-}
-
-// cta_group::2 pairs for the 256-wide tiles; `m_sub` = 128-row sub-tiles of the problem.  IGGT_PAIR is a bit mask over
-// the callers (1 residual, 2 qkv, 4 plain store, 8 convolution; 0 = one CTA per tile everywhere).  Measured on the
-// C2 step (profiles/r01_ncu_notes.md): pairs win for the residual / qkv / conv epilogues (-1.4 ms per step) and lose
-// ~3 % on the GELU store epilogue, whose two coupled epilogues gate the pair's next tile - hence the default 11.
-enum PairUser : int { PAIR_RESID = 1, PAIR_QKV = 2, PAIR_STORE = 4, PAIR_CONV = 8 };
-inline bool use_pair(int user, int bn, int m_sub) {
-  static const int v = [] { const char* e = getenv("IGGT_PAIR"); return e ? atoi(e) : 11; }();
-  return (v & user) != 0 && bn == 256 && m_sub >= 2;
-}
+// Pick the N tile: 128 wherever N allows it (a 128 x 128 tile reads 2 x 16 KB of operands per 64-deep k-block for
+// 2 x 64 x 128 x 64 MACs; the 64-wide tile needs the same A bytes for half the work).  Wider tiles do not fit: the
+// 64 x 256 fp32 accumulator of a consumer warpgroup would take all of its registers.
+inline int choose_bn(int /*m_tiles*/, int N) { return N <= 64 ? 64 : 128; }
 
 // The host-side schedule of one GEMM launch, shared by the launchers and by iggt_gemm_plan (unit-tested without a GPU).
 struct GemmPlan {
   int bn;          // N tile
-  int pair;        // cta_group::2 pairs: m_tiles then counts 256-row tile pairs
+  int pair;        // CTA pairs (a 256-row tile shared by two CTAs): not used on sm_90, always 0
   int stream_k;    // residual epilogue only
   int m_tiles, n_tiles, k_blocks;
   int grid;        // CTAs launched
@@ -46,54 +26,39 @@ inline GemmPlan plan_gemm(int epi, int M, int N, int K) {
   g.k_blocks = (K + GEMM_BK - 1) / GEMM_BK;
   g.m_tiles = m_sub;
   const int sms = device_sm_count();
+  g.bn = choose_bn(m_sub, N);
+  if ((epi == EPI_RESID32 || epi == EPI_QKV) && g.bn < 128) g.bn = 128;
   if (epi == EPI_RESID32) {
-    // Stream-K: wide (128 x 256) tiles keep the main loop under the 128 B/clk shared-memory ceiling, and cutting the
-    // (tile, k-block) space into equal ranges removes the wave-quantisation loss (N = 1024 gives only 2.3 waves of
-    // such tiles at M = 10992).  IGGT_STREAMK=0 restores whole-tile scheduling (bit-reproducible accumulation order).
-    // With CTA pairs the unit of scheduling is a 256 x 256 tile on one of SMs/2 pairs.
-    const bool pair256 = use_pair(PAIR_RESID, 256, m_sub);
-    const int m256 = pair256 ? (m_sub + 1) / 2 : m_sub;
-    const int tiles256 = m256 * ((N + 255) / 256);
-    const int workers = pair256 ? sms / 2 : sms;
-    const bool quantised = tiles256 % workers != 0 && tiles256 > workers / 2;
-    g.stream_k = (sk_env && N >= 256 && quantised && (long)tiles256 * g.k_blocks >= 4L * workers) ? 1 : 0;
-    g.bn = g.stream_k ? 256 : choose_bn(m_sub, N);
-    if (g.bn < 128) g.bn = 128;
-    g.pair = use_pair(PAIR_RESID, g.bn, m_sub) ? 1 : 0;
-  } else {
-    g.bn = choose_bn(m_sub, N);
-    if (epi == EPI_QKV && g.bn < 128) g.bn = 128;
-    g.pair = use_pair(epi == EPI_QKV ? PAIR_QKV : PAIR_STORE, g.bn, m_sub) ? 1 : 0;
+    // Stream-K: cutting the (tile, k-block) space into equal ranges removes the wave-quantisation loss (N = 1024 gives
+    // 5.2 waves of 128 x 128 tiles at M = 10992 on 132 SMs).  IGGT_STREAMK=0 restores whole-tile scheduling
+    // (bit-reproducible accumulation order).
+    const int tiles = m_sub * ((N + 127) / 128);
+    const bool quantised = tiles % sms != 0 && tiles > sms / 2;
+    g.stream_k = (sk_env && N >= 128 && quantised && (long)tiles * g.k_blocks >= 4L * sms) ? 1 : 0;
   }
-  if (g.pair) g.m_tiles = (m_sub + 1) / 2;
   g.n_tiles = (N + g.bn - 1) / g.bn;
-  const int workers_max = g.pair ? sms / 2 : sms;
   const int tiles = g.m_tiles * g.n_tiles;
-  int workers = tiles < workers_max ? tiles : workers_max;
-  if (g.stream_k) workers = workers_max;
-  g.grid = workers * (g.pair ? 2 : 1);
+  g.grid = g.stream_k ? sms : (tiles < sms ? tiles : sms);
   return g;
 }
 
-// PAIR: p.num_m_tiles counts 256-row tile pairs and tB's box holds BN/2 weight rows (see gemm.cuh).
-template <int BN, int EPI, bool BF16, bool CONV, bool PAIR = false, int G = (epi_is_qkv(EPI) ? 1 : 2)>
+template <int BN, int EPI, bool BF16, bool CONV>
 inline int launch_gemm_kernel(const CUtensorMap& tA, const CUtensorMap& tB, const CUtensorMap& tC,
                               const GemmParams& p, cudaStream_t stream) {
-  auto kern = gemm_tcgen05_kernel<BN, EPI, BF16, CONV, G, PAIR>;
+  auto kern = gemm_wgmma_kernel<BN, EPI, BF16, CONV>;
   static DeviceOnce once;
-  constexpr int smem = GemmSmem<BN, PAIR>::TOTAL;
+  constexpr int smem = GemmSmem<BN>::TOTAL;
   static_assert(smem <= 232448, "shared memory budget");
   if (once.first()) {
     cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
     if (e != cudaSuccess) { once.reset_current(); return (int)e; }
   }
-  const int workers_max = PAIR ? device_sm_count() / 2 : device_sm_count();
+  const int sms = device_sm_count();
   const int tiles = p.num_m_tiles * p.num_n_tiles;
-  int workers = tiles < workers_max ? tiles : workers_max;
-  if (p.stream_k) workers = workers_max;
+  int workers = tiles < sms ? tiles : sms;
+  if (p.stream_k) workers = sms;
   if (workers <= 0) return 0;
-  return (int)launch_pdl_cluster(kern, dim3(workers * (PAIR ? 2 : 1)), dim3(128 + 128 * G), smem, stream,
-                                 PAIR ? 2 : 1, tA, tB, tC, p);
+  return (int)launch_pdl(kern, dim3(workers), dim3(GEMM_THREADS), smem, stream, tA, tB, tC, p);
 }
 
 }  // namespace iggt

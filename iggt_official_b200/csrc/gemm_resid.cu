@@ -6,14 +6,11 @@
 using namespace iggt;
 
 namespace {
+// the residual and qkv epilogues always run 128-wide tiles (plan_gemm)
 template <int EPI, bool BF16>
-int dispatch_bn(int bn, bool pair, const CUtensorMap& tA, const CUtensorMap& tB, const CUtensorMap& tC,
-                const GemmParams& p, cudaStream_t s) {
-  if (pair) return launch_gemm_kernel<256, EPI, BF16, false, true>(tA, tB, tC, p, s);
-  switch (bn) {
-    case 256: return launch_gemm_kernel<256, EPI, BF16, false>(tA, tB, tC, p, s);
-    default: return launch_gemm_kernel<128, EPI, BF16, false>(tA, tB, tC, p, s);
-  }
+int dispatch_bn(int /*bn*/, const CUtensorMap& tA, const CUtensorMap& tB, const CUtensorMap& tC, const GemmParams& p,
+                cudaStream_t s) {
+  return launch_gemm_kernel<128, EPI, BF16, false>(tA, tB, tC, p, s);
 }
 }  // namespace
 
@@ -27,16 +24,15 @@ extern "C" int iggt_gemm_resid32(const void* A, int64_t lda, const void* W, int6
   p.M = M; p.N = N; p.K = K; p.bias = bias; p.gamma = gamma; p.round_out16 = round_out16;
   const GemmPlan plan = plan_gemm(EPI_RESID32, M, N, K);
   const int bn = plan.bn;
-  const bool pair = plan.pair != 0;
   p.stream_k = plan.stream_k;
   p.num_m_tiles = plan.m_tiles; p.num_n_tiles = plan.n_tiles; p.num_k_blocks = plan.k_blocks;
   const TmDtype dt = dtype ? TM_BF16 : TM_F16;
   CUtensorMap tA, tB, tC;
   if (make_tmap_2d(&tA, dt, A, M, K, lda, GEMM_BK, GEMM_BM)) return -4;
-  if (make_tmap_2d(&tB, dt, W, N, K, ldw, GEMM_BK, pair ? bn / 2 : bn)) return -4;
+  if (make_tmap_2d(&tB, dt, W, N, K, ldw, GEMM_BK, bn)) return -4;
   if (make_tmap_2d(&tC, TM_F32, x, M, N, ldx, 32, GEMM_BM)) return -4;
-  return dtype ? dispatch_bn<EPI_RESID32, true>(bn, pair, tA, tB, tC, p, (cudaStream_t)stream)
-               : dispatch_bn<EPI_RESID32, false>(bn, pair, tA, tB, tC, p, (cudaStream_t)stream);
+  return dtype ? dispatch_bn<EPI_RESID32, true>(bn, tA, tB, tC, p, (cudaStream_t)stream)
+               : dispatch_bn<EPI_RESID32, false>(bn, tA, tB, tC, p, (cudaStream_t)stream);
 }
 
 extern "C" int iggt_gemm_qkv(const void* A, int64_t lda, const void* W, int64_t ldw, void* qkv,
@@ -61,18 +57,17 @@ extern "C" int iggt_gemm_qkv(const void* A, int64_t lda, const void* W, int64_t 
   p.gather_rows = gather_rows > 0 ? gather_rows : M;
   const GemmPlan plan = plan_gemm(EPI_QKV, M, N, K);
   const int bn = plan.bn;
-  const bool pair = plan.pair != 0;
   p.num_m_tiles = plan.m_tiles; p.num_n_tiles = plan.n_tiles; p.num_k_blocks = plan.k_blocks;
   const TmDtype dt = dtype ? TM_BF16 : TM_F16;
   CUtensorMap tA, tB, tC;
   if (make_tmap_2d(&tA, dt, A, M, K, lda, GEMM_BK, GEMM_BM)) return -4;
-  if (make_tmap_2d(&tB, dt, W, N, K, ldw, GEMM_BK, pair ? bn / 2 : bn)) return -4;
+  if (make_tmap_2d(&tB, dt, W, N, K, ldw, GEMM_BK, bn)) return -4;
   if (make_tmap_2d(&tC, dt, qkv, M, N, ldo, 64, GEMM_BM)) return -4;
   if (n_gather > 0)
-    return dtype ? dispatch_bn<EPI_QKV_GATHER, true>(bn, pair, tA, tB, tC, p, (cudaStream_t)stream)
-                 : dispatch_bn<EPI_QKV_GATHER, false>(bn, pair, tA, tB, tC, p, (cudaStream_t)stream);
-  return dtype ? dispatch_bn<EPI_QKV, true>(bn, pair, tA, tB, tC, p, (cudaStream_t)stream)
-               : dispatch_bn<EPI_QKV, false>(bn, pair, tA, tB, tC, p, (cudaStream_t)stream);
+    return dtype ? dispatch_bn<EPI_QKV_GATHER, true>(bn, tA, tB, tC, p, (cudaStream_t)stream)
+                 : dispatch_bn<EPI_QKV_GATHER, false>(bn, tA, tB, tC, p, (cudaStream_t)stream);
+  return dtype ? dispatch_bn<EPI_QKV, true>(bn, tA, tB, tC, p, (cudaStream_t)stream)
+               : dispatch_bn<EPI_QKV, false>(bn, tA, tB, tC, p, (cudaStream_t)stream);
 }
 
 // Tensor maps for the fused K|V gather: dst[i] = address of THIS rank's first row inside rank i's gathered K|V buffer

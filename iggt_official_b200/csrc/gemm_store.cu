@@ -8,14 +8,10 @@ using namespace iggt;
 namespace {
 
 template <int EPI, bool BF16>
-int dispatch_bn(int bn, bool pair, const CUtensorMap& tA, const CUtensorMap& tB, const CUtensorMap& tC,
-                const GemmParams& p, cudaStream_t s) {
-  if (pair) return launch_gemm_kernel<256, EPI, BF16, false, true>(tA, tB, tC, p, s);
-  switch (bn) {
-    case 256: return launch_gemm_kernel<256, EPI, BF16, false>(tA, tB, tC, p, s);
-    case 128: return launch_gemm_kernel<128, EPI, BF16, false>(tA, tB, tC, p, s);
-    default: return launch_gemm_kernel<64, EPI, BF16, false>(tA, tB, tC, p, s);
-  }
+int dispatch_bn(int bn, const CUtensorMap& tA, const CUtensorMap& tB, const CUtensorMap& tC, const GemmParams& p,
+                cudaStream_t s) {
+  if (bn == 64) return launch_gemm_kernel<64, EPI, BF16, false>(tA, tB, tC, p, s);
+  return launch_gemm_kernel<128, EPI, BF16, false>(tA, tB, tC, p, s);
 }
 
 int gemm_common(int epi, const void* A, int64_t lda, const void* W, int64_t ldw, void* out,
@@ -28,28 +24,27 @@ int gemm_common(int epi, const void* A, int64_t lda, const void* W, int64_t ldw,
   p.M = M; p.N = N; p.K = K;
   const GemmPlan plan = plan_gemm(epi, M, N, K);
   const int bn = plan.bn;
-  const bool pair = plan.pair != 0;
   p.num_m_tiles = plan.m_tiles; p.num_n_tiles = plan.n_tiles; p.num_k_blocks = plan.k_blocks;
   const TmDtype dt = dtype ? TM_BF16 : TM_F16;
   CUtensorMap tA, tB, tC;
   if (make_tmap_2d(&tA, dt, A, M, K, lda, GEMM_BK, GEMM_BM)) return -4;
-  if (make_tmap_2d(&tB, dt, W, N, K, ldw, GEMM_BK, pair ? bn / 2 : bn)) return -4;
+  if (make_tmap_2d(&tB, dt, W, N, K, ldw, GEMM_BK, bn)) return -4;
   if (out32) {
     if (make_tmap_2d(&tC, TM_F32, out, M, N, ldo, 32, GEMM_BM)) return -4;
   } else {
     if (make_tmap_2d(&tC, dt, out, M, N, ldo, 64, GEMM_BM)) return -4;
   }
   if (epi == EPI_STORE16) {
-    return dtype ? dispatch_bn<EPI_STORE16, true>(bn, pair, tA, tB, tC, p, stream)
-                 : dispatch_bn<EPI_STORE16, false>(bn, pair, tA, tB, tC, p, stream);
+    return dtype ? dispatch_bn<EPI_STORE16, true>(bn, tA, tB, tC, p, stream)
+                 : dispatch_bn<EPI_STORE16, false>(bn, tA, tB, tC, p, stream);
   }
-  return dtype ? dispatch_bn<EPI_STORE32, true>(bn, pair, tA, tB, tC, p, stream)
-               : dispatch_bn<EPI_STORE32, false>(bn, pair, tA, tB, tC, p, stream);
+  return dtype ? dispatch_bn<EPI_STORE32, true>(bn, tA, tB, tC, p, stream)
+               : dispatch_bn<EPI_STORE32, false>(bn, tA, tB, tC, p, stream);
 }
 
 }  // namespace
 
-// Host-only: the schedule the launchers would use for an (epilogue, M, N, K) problem on this device (148 SMs assumed
+// Host-only: the schedule the launchers would use for an (epilogue, M, N, K) problem on this device (132 SMs assumed
 // when no GPU is visible).  epi: 0 store16, 1 resid32, 2 qkv (N = 3C), 3 store32.
 // out = {bn, pair, stream_k, m_tiles, n_tiles, k_blocks, grid}.
 extern "C" int iggt_gemm_plan(int epi, int M, int N, int K, int* out) {

@@ -41,9 +41,8 @@ __device__ __forceinline__ float2 cvt16x2(uint32_t u) {
   else return __half22float2(*reinterpret_cast<const __half2*>(&u));
 }
 // One CTA per output row (n, oy): the vertical taps / weights are row constants, a thread walks (ox, 8-channel group)
-// items of the row.  The four-tap blend runs on packed fp32 pairs (FMUL2 / FFMA2, same IEEE results as scalar code):
-// the first version of this kernel was issue-bound (ncu: 71 % issue slots, 1.8 TB/s; profiles/r02a_ncu_all_kernels.csv)
-// on 64-bit index arithmetic and scalar blends.
+// items of the row.  Index arithmetic stays 32-bit; the four-tap blend runs on fp32 pairs (same IEEE results as scalar
+// code).
 template <bool BF16>
 __global__ void __launch_bounds__(256)
 upsample_bilinear_kernel(const uint16_t* __restrict__ x, uint16_t* __restrict__ out, int NB, int h, int w,
@@ -333,7 +332,7 @@ small_attention_kernel(const float* __restrict__ qkv, float* __restrict__ out, i
 
 inline unsigned grid_for(int64_t total, int threads = 256) {
   int64_t g = (total + threads - 1) / threads;
-  const int64_t cap = 148 * 16;
+  const int64_t cap = 132 * 16;
   return static_cast<unsigned>(g < cap ? (g > 0 ? g : 1) : cap);
 }
 

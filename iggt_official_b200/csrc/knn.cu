@@ -2,7 +2,7 @@
 //
 // The reference smooths the per-pixel instance features over the k = 20 nearest 3-D points of ALL views before
 // clustering (demo.py:376-378 -> iggt/utils/misc.py:24-78: torch_geometric knn_graph(loop=False) + torch_scatter
-// scatter_mean, on the CPU by default).  B200 design: no tree, no hash grid - points are ordered along a 63-bit
+// scatter_mean, on the CPU by default).  GPU design: no tree, no hash grid - points are ordered along a 63-bit
 // Morton curve (the sort itself is a library radix sort on the host side of the C ABI), cut into tiles of 256
 // consecutive points with an axis-aligned bounding box each, and every tile of queries runs a block-pruned brute-force
 // search: 256 threads = 256 queries, candidate tiles staged in shared memory and broadcast to all threads, a per-thread

@@ -1,7 +1,7 @@
 // Programmatic dependent launch (PDL) helpers.  Every hot kernel does its global-memory-free prologue (mbarrier
-// init, TMEM allocation, tensor-map prefetch), then `griddep_wait()` before it touches global memory, and lets the
+// init, tensor-map prefetch), then `griddep_wait()` before it touches global memory, and lets the
 // next kernel in the stream begin ITS prologue early with `griddep_launch()`.  With ~730 back-to-back launches per
-// forward (each only 5-100 us once the views are sharded over several GPUs) the launch latency and prologues are
+// forward (each short once the views are sharded over several GPUs) the launch latency and prologues are
 // otherwise exposed.  IGGT_PDL=0 falls back to plain stream-ordered launches.
 #pragma once
 #include <cuda_runtime.h>
@@ -39,10 +39,10 @@ struct DeviceOnce {
 inline int device_sm_count() {
   static int n[kMaxDevices] = {};
   const int d = current_device();
-  if (d < 0 || d >= kMaxDevices) return 148;
+  if (d < 0 || d >= kMaxDevices) return 132;
   if (!n[d]) {
     cudaDeviceGetAttribute(&n[d], cudaDevAttrMultiProcessorCount, d);
-    if (n[d] <= 0) n[d] = 148;
+    if (n[d] <= 0) n[d] = 132;
   }
   return n[d];
 }

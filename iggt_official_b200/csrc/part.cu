@@ -1,4 +1,4 @@
-// Kernels of the part (instance-feature) path that are not GEMM-shaped enough for the tcgen05 main loop:
+// Kernels of the part (instance-feature) path that are not GEMM-shaped enough for the wgmma main loop:
 // small-C LayerNorm on 16-bit NHWC rows, the k4/s2/p1 ConvTranspose gather, the two 8x8-window attentions
 // (OCAB with 12x12 overlapping keys + relative-position bias and the reference's scrambled query windows;
 // HAB plain window self-attention), and the CAB channel-attention (squeeze-excite) pieces.
@@ -379,7 +379,7 @@ se_scale_add_kernel(const uint16_t* __restrict__ y0, const uint16_t* __restrict_
 
 inline unsigned grid_cap(int64_t total, int threads = 256) {
   int64_t g = (total + threads - 1) / threads;
-  const int64_t cap = 148 * 16;
+  const int64_t cap = 132 * 16;
   return static_cast<unsigned>(g < cap ? (g > 0 ? g : 1) : cap);
 }
 

@@ -1,7 +1,7 @@
-// Inline-PTX wrappers for the sm_100a features every kernel in this library uses:
-// mbarrier, TMA (cp.async.bulk.tensor), tcgen05 (alloc / mma / commit / ld) and proxy fences.
+// Inline-PTX wrappers for the sm_90a features every kernel in this library uses:
+// mbarrier, TMA (cp.async.bulk.tensor), wgmma (warpgroup MMA from shared-memory descriptors) and proxy fences.
 // Nothing here is a port: the reference (lifuguan/IGGT_official) has no native code on this path
-// (SURVEY.md §2.2); these are the building blocks of the B200-native kernels.
+// (SURVEY.md §2.2); these are the building blocks of the Hopper-native kernels.
 #pragma once
 #include <cuda.h>
 #include <cuda_fp16.h>
@@ -60,12 +60,6 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
 // ---------------------------------------------------------------- fences
 __device__ __forceinline__ void fence_proxy_async_smem() {
   asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-}
-__device__ __forceinline__ void tc_fence_before() {
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-}
-__device__ __forceinline__ void tc_fence_after() {
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
 }
 __device__ __forceinline__ void named_bar_sync(uint32_t id, uint32_t nthreads) {
   asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
@@ -148,141 +142,83 @@ __device__ __forceinline__ void tma_store_wait_all() {
   asm volatile("cp.async.bulk.wait_group %0;" ::"n"(N) : "memory");
 }
 
-// ---------------------------------------------------------------- tcgen05 / TMEM
-template <uint32_t COLS>
-__device__ __forceinline__ void tmem_alloc(uint32_t* smem_dst) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(
-                   smem_u32(smem_dst)),
-               "n"(COLS)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
+// ---------------------------------------------------------------- wgmma (warpgroup MMA)
+// All four warps of a warpgroup issue the same wgmma; the accumulator lives in registers, distributed as:
+// thread t of the warpgroup (warp w = t / 32, lane l) holds rows 16 w + l / 4 and 16 w + l / 4 + 8; for every 8-column
+// block j its fragment elements [4 j, 4 j + 1] are (row, 8 j + 2 (l % 4) + {0, 1}) and [4 j + 2, 4 j + 3] the same
+// columns of row + 8.
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() {
+  asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory");
 }
-template <uint32_t COLS>
-__device__ __forceinline__ void tmem_dealloc(uint32_t addr) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(addr), "n"(COLS)
-               : "memory");
-}
-// D[tmem] (+)= A[smem desc] * B[smem desc]; issued by ONE thread.
-__device__ __forceinline__ void umma_f16(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc,
-                                         uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}\n" ::"r"(d_tmem),
-      "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// arrive on an mbarrier when all previously issued tcgen05.mma of this thread have completed
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(
-                   smem_u32(bar))
-               : "memory");
-}
-// 32 lanes x 32 columns of 32-bit: thread i of the warp gets row (lane_base + i), 32 consecutive columns
-__device__ __forceinline__ void tmem_ld_32x32(uint32_t taddr, uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]),
-        "=r"(r[7]), "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]),
-        "=r"(r[14]), "=r"(r[15]), "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]),
-        "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]),
-        "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr));
-}
-__device__ __forceinline__ void tmem_ld_wait() {
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
+// keeps the compiler from moving accesses of accumulator registers across wgmma_wait
+template <int R>
+__device__ __forceinline__ void reg_fence(float (&d)[R]) {
+#pragma unroll
+  for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
 
-// ---------------------------------------------------------------- CTA pairs (cta_group::2)
-// Two CTAs of a cluster (same TPC) issue ONE tcgen05.mma of M = 256: each holds its own 128 rows of A and HALF of
-// the B tile in shared memory and receives its 128 accumulator rows in its own TMEM.  Only the rank-0 CTA issues
-// the MMA; TMA loads of both CTAs signal rank 0's "full" barrier, and commits are multicast to both CTAs.
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-  uint32_t r;
-  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-  return r;
+// accumulator operand lists of the wrappers below: 8 fp32 fragment registers per macro
+#define IGGT_D8(o) "+f"(d[o]), "+f"(d[o + 1]), "+f"(d[o + 2]), "+f"(d[o + 3]), "+f"(d[o + 4]), "+f"(d[o + 5]), \
+                   "+f"(d[o + 6]), "+f"(d[o + 7])
+// D (+)= A[smem desc] * B[smem desc], both operands K-major; d: this thread's accumulator fragment
+#define IGGT_WGMMA_SS_32(T)                                                                                     \
+  asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %18, 0;\n\t"                                               \
+               "wgmma.mma_async.sync.aligned.m64n32k16.f32." T "." T " {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, %16, %17, p, 1, 1, 0, 0;\n\t}\n" \
+               : IGGT_D8(0), IGGT_D8(8)                                                                                          \
+               : "l"(a_desc), "l"(b_desc), "r"(accumulate))
+template <bool BF16>
+__device__ __forceinline__ void wgmma_m64n32k16_ss(float (&d)[16], uint64_t a_desc, uint64_t b_desc, uint32_t accumulate) {
+  if constexpr (BF16) IGGT_WGMMA_SS_32("bf16");
+  else IGGT_WGMMA_SS_32("f16");
 }
-__device__ __forceinline__ void cluster_sync_all() {
-  asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
+#define IGGT_WGMMA_SS_64(T)                                                                                     \
+  asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"                                               \
+               "wgmma.mma_async.sync.aligned.m64n64k16.f32." T "." T " {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1, 0, 0;\n\t}\n" \
+               : IGGT_D8(0), IGGT_D8(8), IGGT_D8(16), IGGT_D8(24)                                                                                          \
+               : "l"(a_desc), "l"(b_desc), "r"(accumulate))
+template <bool BF16>
+__device__ __forceinline__ void wgmma_m64n64k16_ss(float (&d)[32], uint64_t a_desc, uint64_t b_desc, uint32_t accumulate) {
+  if constexpr (BF16) IGGT_WGMMA_SS_64("bf16");
+  else IGGT_WGMMA_SS_64("f16");
 }
-// shared::cluster address of `p` (a shared::cta pointer) inside CTA `rank` of the cluster
-__device__ __forceinline__ uint32_t mapa_u32(const void* p, uint32_t rank) {
-  uint32_t r;
-  asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(smem_u32(p)), "r"(rank));
-  return r;
+#define IGGT_WGMMA_SS_128(T)                                                                                     \
+  asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"                                               \
+               "wgmma.mma_async.sync.aligned.m64n128k16.f32." T "." T " {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1, 0, 0;\n\t}\n" \
+               : IGGT_D8(0), IGGT_D8(8), IGGT_D8(16), IGGT_D8(24), IGGT_D8(32), IGGT_D8(40), IGGT_D8(48), IGGT_D8(56)                                                                                          \
+               : "l"(a_desc), "l"(b_desc), "r"(accumulate))
+template <bool BF16>
+__device__ __forceinline__ void wgmma_m64n128k16_ss(float (&d)[64], uint64_t a_desc, uint64_t b_desc, uint32_t accumulate) {
+  if constexpr (BF16) IGGT_WGMMA_SS_128("bf16");
+  else IGGT_WGMMA_SS_128("f16");
 }
-__device__ __forceinline__ void mbar_arrive_cluster(uint32_t cluster_addr) {
-  asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" ::"r"(cluster_addr) : "memory");
-}
-// TMA loads whose completion bytes are credited to an mbarrier of the PEER-or-own CTA (shared::cluster address)
-__device__ __forceinline__ void tma_load_2d_pair(void* smem, const CUtensorMap* m, uint32_t bar_cluster_addr,
-                                                 int32_t c0, int32_t c1) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes"
-      " [%0], [%1, {%3, %4}], [%2];" ::"r"(smem_u32(smem)),
-      "l"(reinterpret_cast<uint64_t>(m)), "r"(bar_cluster_addr), "r"(c0), "r"(c1)
-      : "memory");
-}
-__device__ __forceinline__ void tma_load_4d_pair(void* smem, const CUtensorMap* m, uint32_t bar_cluster_addr,
-                                                 int32_t c0, int32_t c1, int32_t c2, int32_t c3) {
-  asm volatile(
-      "cp.async.bulk.tensor.4d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes"
-      " [%0], [%1, {%3, %4, %5, %6}], [%2];" ::"r"(smem_u32(smem)),
-      "l"(reinterpret_cast<uint64_t>(m)), "r"(bar_cluster_addr), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
-      : "memory");
-}
-template <uint32_t COLS>
-__device__ __forceinline__ void tmem_alloc_pair(uint32_t* smem_dst) {
-  asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_dst)),
-               "n"(COLS)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-}
-template <uint32_t COLS>
-__device__ __forceinline__ void tmem_dealloc_pair(uint32_t addr) {
-  asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(addr), "n"(COLS) : "memory");
-}
-__device__ __forceinline__ void umma_f16_pair(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc,
-                                              uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t}\n" ::"r"(d_tmem),
-      "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// arrive on the mbarrier at the same shared-memory offset in BOTH CTAs of the pair
-__device__ __forceinline__ void umma_commit_pair(uint64_t* bar) {
-  asm volatile(
-      "tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(
-          smem_u32(bar)),
-      "h"(static_cast<uint16_t>(3))
-      : "memory");
+// D (+)= A[registers] * B[smem desc], B MN-major (transposed); a: the mma.sync-style A fragment of k16
+#define IGGT_WGMMA_RS_TB_64(T)                                                                                   \
+  asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %37, 0;\n\t"                                               \
+               "wgmma.mma_async.sync.aligned.m64n64k16.f32." T "." T " {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, {%32, %33, %34, %35}, %36, p, 1, 1, 1;\n\t}\n" \
+               : IGGT_D8(0), IGGT_D8(8), IGGT_D8(16), IGGT_D8(24)                                                                                          \
+               : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(b_desc), "r"(accumulate))
+template <bool BF16>
+__device__ __forceinline__ void wgmma_m64n64k16_rs_tb(float (&d)[32], const uint32_t (&a)[4], uint64_t b_desc,
+                                                      uint32_t accumulate) {
+  if constexpr (BF16) IGGT_WGMMA_RS_TB_64("bf16");
+  else IGGT_WGMMA_RS_TB_64("f16");
 }
 
 // ---------------------------------------------------------------- descriptors
-// Shared-memory matrix descriptor (cute::UMMA::SmemDescriptor bit layout: start>>4 [0,14),
-// LBO>>4 [16,30), SBO>>4 [32,46), version=1 [46,48), layout_type [61,64); SWIZZLE_128B = 2).
-// K-major, 128-byte swizzle: rows are 128 B (64 x 16-bit), 8-row groups are 1024 B apart.
+// wgmma shared-memory matrix descriptor (sm_90): start>>4 [0,14), LBO>>4 [16,30), SBO>>4 [32,46), layout type [62,64)
+// (1 = SWIZZLE_128B).  128-byte swizzle: rows of 128 B (64 x 16-bit), 8-row atoms 1024 B apart (SBO); for a K-major
+// operand the k16 steps inside an atom advance the start address by 32 B, for an MN-major operand SBO is the distance
+// between groups of 8 k-rows.  Tiles must be 1024-byte aligned (base offset 0).
 __device__ __forceinline__ uint64_t make_desc_sw128(uint32_t smem_addr, uint32_t sbo_bytes) {
   uint64_t d = 0;
   d |= static_cast<uint64_t>((smem_addr & 0x3FFFF) >> 4);
   d |= static_cast<uint64_t>(1) << 16;                       // LBO (unused for 128B swizzle)
   d |= static_cast<uint64_t>((sbo_bytes >> 4) & 0x3FFF) << 32;
-  d |= static_cast<uint64_t>(1) << 46;                       // descriptor version (Blackwell)
-  d |= static_cast<uint64_t>(2) << 61;                       // SWIZZLE_128B
+  d |= static_cast<uint64_t>(1) << 62;                       // SWIZZLE_128B
   return d;
-}
-// Instruction descriptor for kind::f16 (cute::UMMA::InstrDescriptor): c_format F32=1 at [4,6),
-// a_format [7,10), b_format [10,13) (0 = fp16, 1 = bf16), a_major bit 15, b_major bit 16
-// (0 = K-major, 1 = MN-major), N>>3 at [17,23), M>>4 at [24,29).
-__host__ __device__ constexpr uint32_t make_idesc_f16(uint32_t M, uint32_t N, bool bf16,
-                                                      bool a_mn_major, bool b_mn_major) {
-  return (1u << 4) | ((bf16 ? 1u : 0u) << 7) | ((bf16 ? 1u : 0u) << 10) |
-         ((a_mn_major ? 1u : 0u) << 15) | ((b_mn_major ? 1u : 0u) << 16) | ((N >> 3) << 17) |
-         ((M >> 4) << 24);
 }
 
 // ---------------------------------------------------------------- small math helpers
@@ -313,34 +249,15 @@ __device__ __forceinline__ float ex2_approx(float x) {
   asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
   return y;
 }
-// Packed fp32 pairs (sm_100 FFMA2 / FADD2 / FMUL2): two IEEE-rounded fp32 operations per issue slot.
+// fp32 pairs: two IEEE-rounded fp32 operations (the pair form keeps the callers' arithmetic explicit and in order).
 __device__ __forceinline__ float2 ffma2(float2 a, float2 b, float2 c) {
-  uint64_t ra, rb, rc, rd;
-  asm("mov.b64 %0, {%1, %2};" : "=l"(ra) : "f"(a.x), "f"(a.y));
-  asm("mov.b64 %0, {%1, %2};" : "=l"(rb) : "f"(b.x), "f"(b.y));
-  asm("mov.b64 %0, {%1, %2};" : "=l"(rc) : "f"(c.x), "f"(c.y));
-  asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(rd) : "l"(ra), "l"(rb), "l"(rc));
-  float2 d;
-  asm("mov.b64 {%0, %1}, %2;" : "=f"(d.x), "=f"(d.y) : "l"(rd));
-  return d;
+  return make_float2(__fmaf_rn(a.x, b.x, c.x), __fmaf_rn(a.y, b.y, c.y));
 }
 __device__ __forceinline__ float2 fadd2(float2 a, float2 b) {
-  uint64_t ra, rb, rd;
-  asm("mov.b64 %0, {%1, %2};" : "=l"(ra) : "f"(a.x), "f"(a.y));
-  asm("mov.b64 %0, {%1, %2};" : "=l"(rb) : "f"(b.x), "f"(b.y));
-  asm("add.rn.f32x2 %0, %1, %2;" : "=l"(rd) : "l"(ra), "l"(rb));
-  float2 d;
-  asm("mov.b64 {%0, %1}, %2;" : "=f"(d.x), "=f"(d.y) : "l"(rd));
-  return d;
+  return make_float2(__fadd_rn(a.x, b.x), __fadd_rn(a.y, b.y));
 }
 __device__ __forceinline__ float2 fmul2(float2 a, float2 b) {
-  uint64_t ra, rb, rd;
-  asm("mov.b64 %0, {%1, %2};" : "=l"(ra) : "f"(a.x), "f"(a.y));
-  asm("mov.b64 %0, {%1, %2};" : "=l"(rb) : "f"(b.x), "f"(b.y));
-  asm("mul.rn.f32x2 %0, %1, %2;" : "=l"(rd) : "l"(ra), "l"(rb));
-  float2 d;
-  asm("mov.b64 {%0, %1}, %2;" : "=f"(d.x), "=f"(d.y) : "l"(rd));
-  return d;
+  return make_float2(__fmul_rn(a.x, b.x), __fmul_rn(a.y, b.y));
 }
 // Exact-erf GELU to ~2e-7 absolute: erf via Abramowitz-Stegun 7.1.26 (|err| <= 1.5e-7), branch-free,
 // 2 MUFU + ~12 FMA-pipe instructions (libdevice erff is ~3x longer and serialises the epilogue).
@@ -358,9 +275,8 @@ __device__ __forceinline__ float gelu_fast(float x) {
   return fmaf(hx, copysignf(erf_abs, x), hx);
 }
 
-// Two GELUs at once on packed fp32 pairs: the same Abramowitz-Stegun evaluation as gelu_fast, operation for operation
-// (every step is an IEEE-rounded fp32 multiply / fma, the two MUFU calls per element are unchanged), in ~half the
-// issue slots.
+// Two GELUs at once on fp32 pairs: the same Abramowitz-Stegun evaluation as gelu_fast, operation for operation
+// (every step is an IEEE-rounded fp32 multiply / fma, the two MUFU calls per element are unchanged).
 __device__ __forceinline__ float2 gelu_fast2(float2 x) {
   const float2 ax = make_float2(fabsf(x.x), fabsf(x.y));
   const float2 z = fmul2(ax, make_float2(0.70710678118654752440f, 0.70710678118654752440f));
@@ -384,8 +300,7 @@ __device__ __forceinline__ float2 gelu_fast2(float2 x) {
 // least-squares fit of log2(erfc(z)) / z, max error 3e-5 in log2 units), so
 //   gelu(x) = 0.5 x + 0.5 |x| (1 - erfc(z)) = hx - na + na * e,   na = -|hx|,  e = erfc(z),  hx = x / 2.
 // Absolute error <= 1.6e-6, relative error <= 2.1e-5 wherever the result is an fp16 normal (the result is rounded to
-// 16 bit right after, half an fp16 ulp = 2.4e-4).  Packed: 9 FFMA2 / FMUL2 + 2 LOP + 2 FMNMX + 2 MUFU per pair, against
-// 4 MUFU for gelu_fast2 (reciprocal + exponential).
+// 16 bit right after, half an fp16 ulp = 2.4e-4).  2 MUFU per pair, against 4 for gelu_fast2 (reciprocal + exponential).
 __device__ __forceinline__ float2 gelu_erfc2(float2 x) {
   const float2 hx = fmul2(x, make_float2(0.5f, 0.5f));
   const float2 na = make_float2(__uint_as_float(__float_as_uint(hx.x) | 0x80000000u),

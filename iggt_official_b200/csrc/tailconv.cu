@@ -4,16 +4,16 @@
 // (iggt/heads/part_head.py:240-243).
 //
 // Why a dedicated kernel: the generic implicit-GEMM convolution (gemm.cuh) loads one TMA box per tap, i.e. re-reads
-// this 550 MB input (8 x 518 x 518 x 128, 16-bit) nine times through L2 for 0.16 TFLOP of work (0.8 ms per launch,
-// profiles/r01_ncu_notes.md), then writes a 32-channel 16-bit map that a second kernel reads back.  Here:
+// this 550 MB input (8 x 518 x 518 x 128, 16-bit) nine times through L2 for 0.16 TFLOP of work, then writes a 32-channel 16-bit map that a second kernel reads back.  Here:
 //   * tall boxes: an output tile is 8 (x) x 16 (y) pixels = 128 GEMM rows.  For each x-shift dx in {-1,0,1} and each
 //     64-channel block ONE box {64 ch, 8 px, 18 rows} is loaded (TMA zero-fills the halo).  A box row (8 px x 128 B)
 //     is exactly one 128B-swizzle atom, so the A operand of tap (dy, dx) is the same box at a (dy+1)*1024-byte
-//     offset - an ordinary atom-aligned UMMA descriptor.  6 boxes (108 KB) per tile instead of 18 taps (288 KB);
+//     offset - an ordinary atom-aligned wgmma descriptor.  6 boxes (108 KB) per tile instead of 18 taps (288 KB);
 //   * the 9 x 2 weight tiles (32 couts x 64 ch, 72 KB) stay resident in shared memory for the whole persistent CTA;
-//   * the 32 accumulators of a pixel never leave registers: + bias, ReLU, the 32 -> OC 1x1 product in fp32 and
-//     exp / sign*expm1 / 1+exp are applied by the epilogue thread that owns the pixel, which writes the fp32 outputs
-//     directly (no 16-bit rounding of the 32-channel map, no second pass).
+//   * two consumer warpgroups issue the wgmma of 64 pixels each; the 32 fp32 accumulators of a pixel go through a small
+//     shared-memory tile to the thread that owns the pixel: + bias, ReLU, the 32 -> OC 1x1 product in fp32 and
+//     exp / sign*expm1 / 1+exp are applied there and the fp32 outputs written directly (no 16-bit rounding of the
+//     32-channel map, no second pass).
 // Bound: HBM (input read once, 2 B x 128 per pixel in, <= 32 B per pixel out); algorithmic bytes per pixel 256 + 4*OC.
 #include <stdlib.h>
 #include "ptx.cuh"
@@ -31,7 +31,10 @@ constexpr int TC_B_BYTES = TC_N * 128;               // 4 KB per (tap, channel b
 constexpr int TC_STAGES = 7;
 constexpr int TC_MAXOC = 8;
 constexpr int TC_VEC_BYTES = (TC_N + TC_MAXOC * TC_N + TC_MAXOC) * 4;     // bias32 | w2[OC][32] | b2[OC]
-constexpr int TC_SMEM = 18 * TC_B_BYTES + TC_STAGES * TC_A_BYTES + 256 + ((TC_VEC_BYTES + 127) / 128) * 128;
+constexpr int TC_ACC_LD = TC_N + 8;                  // fp32 accumulator tile row pitch (conflict-free fragment stores)
+constexpr int TC_ACC_BYTES = 128 * TC_ACC_LD * 4;
+constexpr int TC_THREADS = 384;                       // producer warpgroup + 2 consumer warpgroups
+constexpr int TC_SMEM = 18 * TC_B_BYTES + TC_STAGES * TC_A_BYTES + TC_ACC_BYTES + 256 + ((TC_VEC_BYTES + 127) / 128) * 128;
 static_assert(TC_SMEM <= 232448, "shared memory budget");
 static_assert(TC_A_BYTES % 1024 == 0 && TC_B_BYTES % 1024 == 0, "128B-swizzle atoms need 1024-byte aligned tiles");
 
@@ -49,19 +52,17 @@ struct TailConvParams {
 };
 
 template <bool BF16>
-__global__ void __launch_bounds__(256, 1)
+__global__ void __launch_bounds__(TC_THREADS, 1)
 tailconv_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const TailConvParams p) {
   extern __shared__ __align__(1024) uint8_t smem[];
   if ((smem_u32(smem) & 1023u) != 0) __trap();
   uint8_t* smem_b = smem;                                  // [tap 0..8][cb 0..1] weight tiles
   uint8_t* smem_a = smem + 18 * TC_B_BYTES;                // ring of tall boxes
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem_a + TC_STAGES * TC_A_BYTES);
+  float* acc_tile = reinterpret_cast<float*>(smem_a + TC_STAGES * TC_A_BYTES);   // [128 pixels][TC_ACC_LD]
+  uint64_t* bars = reinterpret_cast<uint64_t*>(reinterpret_cast<uint8_t*>(acc_tile) + TC_ACC_BYTES);
   uint64_t* a_full = bars;
   uint64_t* a_empty = bars + TC_STAGES;
   uint64_t* b_full = bars + 2 * TC_STAGES;
-  uint64_t* tfull = b_full + 1;
-  uint64_t* tempty = tfull + 2;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tempty + 2);
   float* vec = reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(bars) + 256);
   float* s_bias = vec;                                     // [32]
   float* s_w2 = vec + TC_N;                                // [OC][32]
@@ -70,16 +71,11 @@ tailconv_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   if (warp == 0 && lane == 0) { tma_prefetch_desc(&tmA); tma_prefetch_desc(&tmB); }
   if (warp == 1 && lane == 0) {
-    for (int i = 0; i < TC_STAGES; ++i) { mbar_init(&a_full[i], 1); mbar_init(&a_empty[i], 1); }
+    for (int i = 0; i < TC_STAGES; ++i) { mbar_init(&a_full[i], 1); mbar_init(&a_empty[i], 2); }   // 2 consumers
     mbar_init(b_full, 1);
-    for (int i = 0; i < 2; ++i) { mbar_init(&tfull[i], 1); mbar_init(&tempty[i], 4); }
     fence_barrier_init();
   }
-  if (warp == 2) tmem_alloc<64>(tmem_slot);                // two accumulator stages of 32 columns
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
   griddep_wait();
   griddep_launch();
 
@@ -91,8 +87,8 @@ tailconv_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
     x0 = (r % p.tiles_x) * TC_TW;
   };
 
-  if (warp == 0) {
-    if (lane == 0) {
+  if (warp < 4) {
+    if (warp == 0 && lane == 0) {
       // weights once: 18 boxes of {64 ch, 32 couts} on one barrier
       mbar_expect_tx(b_full, 18 * TC_B_BYTES);
       for (int tap = 0; tap < 9; ++tap)
@@ -111,71 +107,80 @@ tailconv_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
           }
       }
     }
-  } else if (warp == 1) {
-    if (lane == 0) {
-      constexpr uint32_t idesc = make_idesc_f16(128, TC_N, BF16, false, false);
-      mbar_wait(b_full, 0);
-      int st = 0; uint32_t ph = 0;
-      int acc = 0; uint32_t acc_ph = 0;
-      for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x) {
-        mbar_wait(&tempty[acc], acc_ph ^ 1);
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + acc * TC_N;
-        bool first = true;
-        for (int dx = -1; dx <= 1; ++dx)
-          for (int cb = 0; cb < 2; ++cb) {
-            mbar_wait(&a_full[st], ph);
-            tc_fence_after();
-            const uint32_t a_base = smem_u32(smem_a + st * TC_A_BYTES);
-#pragma unroll
-            for (int dy = -1; dy <= 1; ++dy) {
-              const int tap = (dy + 1) * 3 + (dx + 1);
-              const uint32_t a_addr = a_base + (dy + 1) * (TC_TW * 128);      // (dy + 1) box rows down: 1024 B each
-              const uint32_t b_addr = smem_u32(smem_b + (tap * 2 + cb) * TC_B_BYTES);
-#pragma unroll
-              for (int k = 0; k < 4; ++k) {
-                umma_f16(d_tmem, make_desc_sw128(a_addr + k * 32, 1024), make_desc_sw128(b_addr + k * 32, 1024), idesc,
-                         first ? 0u : 1u);
-                first = false;
-              }
-            }
-            umma_commit(&a_empty[st]);
-            if (++st == TC_STAGES) { st = 0; ph ^= 1; }
-          }
-        umma_commit(&tfull[acc]);
-        if (++acc == 2) { acc = 0; acc_ph ^= 1; }
-      }
-    }
-  } else if (warp >= 4) {
-    // ---------------------------------------------------------------- epilogue: thread = pixel of the tile
-    const int et = threadIdx.x - 128;
-    for (int i = et; i < TC_N; i += 128) s_bias[i] = p.bias ? p.bias[i] : 0.f;
+  } else {
+    // ---------------------------------------------------------------- consumers: warpgroup cw = GEMM rows [64 cw, +64)
+    const int cw = (warp - 4) >> 2;
+    const int gtid = threadIdx.x & 127;
+    const int ew = (warp - 4) & 3;
+    for (int i = threadIdx.x - 128; i < TC_N; i += 256) s_bias[i] = p.bias ? p.bias[i] : 0.f;
     if (p.w2) {
-      for (int i = et; i < p.OC * TC_N; i += 128) s_w2[i] = p.w2[i];
-      for (int i = et; i < p.OC; i += 128) s_b2[i] = p.b2[i];
+      for (int i = threadIdx.x - 128; i < p.OC * TC_N; i += 256) s_w2[i] = p.w2[i];
+      for (int i = threadIdx.x - 128; i < p.OC; i += 256) s_b2[i] = p.b2[i];
     }
-    named_bar_sync(1, 128);
-    const int ew = warp & 3;
-    const int row = ew * 32 + lane;                        // GEMM row = pixel (yl, xl) of the tile
+    named_bar_sync(1, 256);
+    const int row = cw * 64 + gtid;                        // epilogue (gtid < 64): GEMM row = pixel (yl, xl) of the tile
     const int xl = row % TC_TW, yl = row / TC_TW;
     const int64_t hw = static_cast<int64_t>(p.H) * p.W;
-    int acc = 0; uint32_t acc_ph = 0;
+    const uint32_t bar_id = 2 + cw;
+    mbar_wait(b_full, 0);
+    int st = 0; uint32_t ph = 0;
     for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x) {
       int img, y0, x0;
       decode(tile, img, y0, x0);
-      mbar_wait(&tfull[acc], acc_ph);
-      tc_fence_after();
-      uint32_t r[32];
-      tmem_ld_32x32(tmem_base + (static_cast<uint32_t>(ew * 32) << 16) + acc * TC_N, r);
-      tmem_ld_wait();
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&tempty[acc]);
+      float acc[TC_N / 2];
+#pragma unroll
+      for (int i = 0; i < TC_N / 2; ++i) acc[i] = 0.f;
+      bool first = true;
+      int prev = -1;
+      for (int dx = -1; dx <= 1; ++dx)
+        for (int cb = 0; cb < 2; ++cb) {
+          mbar_wait(&a_full[st], ph);
+          const uint32_t a_base = smem_u32(smem_a + st * TC_A_BYTES) + cw * (8 * TC_TW * 128);   // 8 box rows down
+          wgmma_fence();
+#pragma unroll
+          for (int dy = -1; dy <= 1; ++dy) {
+            const int tap = (dy + 1) * 3 + (dx + 1);
+            const uint32_t a_addr = a_base + (dy + 1) * (TC_TW * 128);      // (dy + 1) box rows down: 1024 B each
+            const uint32_t b_addr = smem_u32(smem_b + (tap * 2 + cb) * TC_B_BYTES);
+#pragma unroll
+            for (int k = 0; k < 4; ++k) {
+              wgmma_m64n32k16_ss<BF16>(acc, make_desc_sw128(a_addr + k * 32, 1024), make_desc_sw128(b_addr + k * 32, 1024),
+                                       first ? 0u : 1u);
+              first = false;
+            }
+          }
+          wgmma_commit();
+          wgmma_wait<1>();                                 // the previous box's MMAs have retired: free its slot
+          if (prev >= 0 && gtid == 0) mbar_arrive(&a_empty[prev]);
+          prev = st;
+          if (++st == TC_STAGES) { st = 0; ph ^= 1; }
+        }
+      wgmma_wait<0>();
+      reg_fence(acc);
+      if (gtid == 0) mbar_arrive(&a_empty[prev]);
+      // accumulator fragments -> this warpgroup's 64 rows of the fp32 tile
+      named_bar_sync(bar_id, 128);                         // the previous tile's rows have been read
+      {
+        float* const d0 = acc_tile + (cw * 64 + ew * 16 + (lane >> 2)) * TC_ACC_LD + 2 * (lane & 3);
+#pragma unroll
+        for (int j = 0; j < TC_N / 8; ++j) {
+          *reinterpret_cast<float2*>(d0 + 8 * j) = make_float2(acc[4 * j], acc[4 * j + 1]);
+          *reinterpret_cast<float2*>(d0 + 8 * TC_ACC_LD + 8 * j) = make_float2(acc[4 * j + 2], acc[4 * j + 3]);
+        }
+      }
+      named_bar_sync(bar_id, 128);
+      if (gtid >= 64) continue;
+      float r[TC_N];
+#pragma unroll
+      for (int i = 0; i < TC_N; i += 4) {
+        const float4 a = *reinterpret_cast<const float4*>(acc_tile + row * TC_ACC_LD + i);
+        r[i] = a.x; r[i + 1] = a.y; r[i + 2] = a.z; r[i + 3] = a.w;
+      }
       const int y = y0 + yl, x = x0 + xl;
       if (y < p.H && x < p.W) {
         float f[TC_N];
 #pragma unroll
-        for (int i = 0; i < TC_N; ++i) f[i] = relu_nan(__uint_as_float(r[i]) + s_bias[i]);     // conv bias + ReLU
+        for (int i = 0; i < TC_N; ++i) f[i] = relu_nan(r[i] + s_bias[i]);     // conv bias + ReLU
         const int64_t pix = (static_cast<int64_t>(img) * p.H + y) * p.W + x;
         if (!p.w2) {
           uint16_t* dst = reinterpret_cast<uint16_t*>(p.out16) + pix * TC_N;
@@ -215,14 +220,7 @@ tailconv_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
           }
         }
       }
-      if (++acc == 2) { acc = 0; acc_ph ^= 1; }
     }
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 2) {
-    tc_fence_after();
-    tmem_dealloc<64>(tmem_base);
   }
 }
 
@@ -236,7 +234,7 @@ int launch_tailconv(const CUtensorMap& tA, const CUtensorMap& tB, const TailConv
   }
   const int sms = device_sm_count();
   const int grid = p.total_tiles < sms ? p.total_tiles : sms;
-  return (int)launch_pdl(kern, dim3(grid), dim3(256), TC_SMEM, stream, tA, tB, p);
+  return (int)launch_pdl(kern, dim3(grid), dim3(TC_THREADS), TC_SMEM, stream, tA, tB, p);
 }
 
 }  // namespace iggt

@@ -233,7 +233,7 @@ layernorm_rows_kernel(const float* __restrict__ x, int64_t ldx, int C, const flo
 
 inline unsigned cap_grid(int64_t work, int per_block) {
   const int64_t g = (work + per_block - 1) / per_block;
-  return static_cast<unsigned>(g < 1 ? 1 : (g > 148 * 16 ? 148 * 16 : g));
+  return static_cast<unsigned>(g < 1 ? 1 : (g > 132 * 16 ? 132 * 16 : g));
 }
 
 }  // namespace iggt

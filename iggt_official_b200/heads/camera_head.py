@@ -1,4 +1,4 @@
-"""B200-native camera head: iterative pose refinement on the S camera tokens
+"""Hopper-native camera head: iterative pose refinement on the S camera tokens
 (reference: iggt/heads/camera_head.py:83-154, iggt/heads/head_act.py:12-35).
 
 M = B*S rows of width 2048 against 216 M parameters: every Linear is a weight stream (fp32 activations, 16-bit

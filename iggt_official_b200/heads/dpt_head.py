@@ -1,10 +1,10 @@
-"""B200-native DPT dense head (depth / 3-D points, and the feature pyramid the part head consumes).
+"""Hopper-native DPT dense head (depth / 3-D points, and the feature pyramid the part head consumes).
 
 Interface of the reference `iggt.heads.dpt_head.DPTHead.forward(aggregated_tokens_list, images,
 patch_start_idx, frames_chunk_size)` (iggt/heads/dpt_head.py:130-190); returns (preds, conf) or, with
 `use_point_feat`, (preds, conf, (out2, out3, out4)) where the feature maps are NHWC 16-bit tensors.
 
-All activations are NHWC 16-bit; every convolution runs on the tcgen05 implicit-GEMM kernel
+All activations are NHWC 16-bit; every convolution runs on the wgmma implicit-GEMM kernel
 (`iggt_conv_nhwc` / `iggt_gemm_store16`) with fp32 accumulation.  Fusions relative to the reference graph:
   * ResidualConvUnit's in-place ReLU (SURVEY F10): producers emit relu(x) directly (act / act_post flags),
     the skip-adds ride in the conv epilogue (resid, resid2);

@@ -1,4 +1,4 @@
-"""B200-native part (instance-feature) path.
+"""Hopper-native part (instance-feature) path.
 
 `PartAdaptor`  = reference `SamProjector` (iggt/heads/adaptor.py:140-226): LN -> 1x1 proj -> per-level resize
                  stacks (ConvTranspose k4/s2/p1, k2/s2, Conv3x3/s2, `Projects` with eval-mode BatchNorm folded
@@ -9,7 +9,7 @@
                  overlapping-window cross attention SwinCA/OCAB at (4g)^2, then SwinSA/HAB at (8g)^2, bilinear
                  to HxW, 3x3 -> ReLU -> 1x1 -> 8 raw channels [B,S,8,H,W].
                  `cross_attention_1` never reaches the output (SURVEY F4) and is not evaluated.
-All convolutions / Linear layers run on the tcgen05 GEMM / implicit-GEMM kernels; window attentions, small-C
+All convolutions / Linear layers run on the wgmma GEMM / implicit-GEMM kernels; window attentions, small-C
 LayerNorms and the channel-attention run on the kernels in csrc/part.cu.
 """
 from typing import List

@@ -1,4 +1,4 @@
-"""B200-native track head (SURVEY.md 8f row 4): the `query_points` branch of `IGGT.forward` / `VGGT.forward`.
+"""Hopper-native track head (SURVEY.md 8f row 4): the `query_points` branch of `IGGT.forward` / `VGGT.forward`.
 
 Interface of the reference `iggt.heads.track_head.TrackHead.forward(aggregated_tokens_list, images, patch_start_idx,
 query_points, iters)` (iggt/heads/track_head.py:73-109) -> (list of per-iteration tracks [B,S,N,2] in image pixels,
@@ -9,7 +9,7 @@ visibility [B,S,N], confidence [B,S,N]).
 * Tracker = BaseTrackerPredictor (track_modules/base_track_predictor.py:85-209).  Rows of every per-track tensor are
   ordered (scene, track, frame), which is the layout the update transformer's time attention wants.  The correlation
   lookup never builds the correlation volume (`ops.corr_sample`); the update transformer (blocks.py:19-144) runs on the
-  tcgen05 GEMM / attention kernels with its 48-wide heads zero-padded to 64 (padded q/k columns add nothing to the
+  wgmma GEMM / attention kernels with its 48-wide heads zero-padded to 64 (padded q/k columns add nothing to the
   scores, padded v columns are dropped by the padded out_proj) and a fp32 token stream like the trunk.
 The reference evaluates this head in fp32 / TF32; GEMM operands here are 16-bit with fp32 accumulation.
 """

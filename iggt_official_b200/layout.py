@@ -1,6 +1,6 @@
 """Checkpoint (`state_dict`) layout of the reference `IGGT` module tree and a builder that materialises
 it as nested nn.Modules, so `load_state_dict` / `utils/model.py:align_and_update_state_dicts` /
-`PyTorchModelHubMixin` keep working against the B200 implementation (SURVEY.md section 8b, Appendix C).
+`PyTorchModelHubMixin` keep working against the native implementation (SURVEY.md section 8b, Appendix C).
 
 `state_layout.json` lists the 2053 (name, shape, dtype) entries of `IGGT().state_dict()` for the default
 constructor arguments (img_size 518, patch 14, embed_dim 1024); tests/test_layout.py checks it against the
@@ -20,7 +20,7 @@ _BUFFER_LEAVES = ("running_mean", "running_var", "num_batches_tracked", "relativ
 
 def load_layout(img_size=518, patch_size=14, embed_dim=1024):
     if patch_size != 14 or embed_dim != 1024:
-        raise NotImplementedError("the B200 kernels are specialised for patch_size=14, embed_dim=1024 "
+        raise NotImplementedError("the native kernels are specialised for patch_size=14, embed_dim=1024 "
                                   "(the only configuration the reference checkpoint uses)")
     with open(os.path.join(_HERE, "state_layout.json")) as f:
         entries = [(k, tuple(s), getattr(torch, d)) for k, s, d in json.load(f)]

@@ -1,4 +1,4 @@
-"""B200-native Aggregator: DINOv2 ViT-L/14-reg tokeniser + 24 x (frame, global) attention blocks.
+"""Hopper-native Aggregator: DINOv2 ViT-L/14-reg tokeniser + 24 x (frame, global) attention blocks.
 
 Same interface as the reference `iggt.models.aggregator.Aggregator` (iggt/models/aggregator.py:186-275):
 `forward(images[B,S,3,H,W]) -> (list of 24 [B,S,T,2C] fp32 tensors, patch_start_idx)`; only the layers the
@@ -76,7 +76,7 @@ def _require_cuda(images: torch.Tensor):
     """The product path has no CPU fallback.  (tests/test_model_wiring.py replaces this hook AND every launcher of
     `ops` with PyTorch statements to exercise the host-side graph on the CPU.)"""
     if not images.is_cuda:
-        raise RuntimeError("iggt_official_b200 runs on CUDA (sm_100a) only; there is no CPU fallback")
+        raise RuntimeError("iggt_official_b200 runs on CUDA (sm_90a) only; there is no CPU fallback")
 
 
 class Aggregator(Node):

@@ -1,6 +1,6 @@
 """Drop-in model classes: `IGGT` and `VGGT` with the reference constructor, `forward(images,
 query_points=None)` signature, output dictionary and `state_dict` layout (iggt/models/vggt.py:14-230),
-running on the sm_100a kernels of this package.
+running on the sm_90a kernels of this package.
 
     from iggt_official_b200.models.vggt import IGGT      # instead of iggt.models.vggt
     model = IGGT(); model.load_state_dict(ckpt, strict=False); model.eval().to("cuda")
@@ -16,7 +16,7 @@ Differences from the reference that a caller can observe:
     exponent range; `model.check_finite = True` makes forward raise FloatingPointError when an output is not
     finite (e.g. a checkpoint whose head activations exceed fp16's 65504) instead of returning inf / nan.
   * S > 12 views works (the reference's frame-chunk path raises TypeError, SURVEY F3).
-  * `query_points` runs the B200 track head (heads/track_head.py, reference iggt/models/vggt.py:220-226) and adds
+  * `query_points` runs the native track head (heads/track_head.py, reference iggt/models/vggt.py:220-226) and adds
     `track`, `vis`, `conf` to the dictionary exactly like the reference; S > 12 works there too.
 """
 from typing import Optional

@@ -1,5 +1,5 @@
 /*
- * iggt_b200.h -- C ABI of the B200-native IGGT inference kernels (libiggt_b200.so).
+ * iggt_b200.h -- C ABI of the Hopper-native (sm_90a) IGGT inference kernels (libiggt_b200.so).
  *
  * The reference (lifuguan/IGGT_official) has no FFI on this path: everything below
  * `IGGT.forward` (iggt/models/vggt.py:149-230) is torch.nn modules.  This header is therefore the
@@ -25,7 +25,7 @@ typedef void* iggt_stream_t; /* cudaStream_t */
 int iggt_device_info(int* sm, int* num_sms);
 const char* iggt_version(void);
 
-/* ---- GEMM family (tcgen05 / TMEM / TMA).  A:[M,K] lda, W:[N,K] ldw (torch Linear layout), 16-bit. */
+/* ---- GEMM family (wgmma / TMA).  A:[M,K] lda, W:[N,K] ldw (torch Linear layout), 16-bit. */
 
 /* out16[M,N] = act(A W^T + bias) (+ addend[(row % add_rows), :]).  act: 0 none, 1 exact-erf GELU,
  * 2 ReLU, 3 LeakyReLU(0.01).  Replaces mlp.fc1 (iggt/layers/mlp.py:35-36), DPT `projects` 1x1 conv +
@@ -78,7 +78,7 @@ int iggt_conv_nhwc(const void* x, const void* Wp, void* out, int NB, int H, int 
                    const void* resid2, int act_post, iggt_stream_t stream);
 
 
-/* ---- Flash attention forward (tcgen05 QK^T / PV, TMEM accumulators, online softmax), head_dim 64.
+/* ---- Flash attention forward (wgmma QK^T / PV, register accumulators, online softmax), head_dim 64.
  * q/k/v/o: token-major [rows, ld] 16-bit, head h in columns [64h, 64h+64).  Sequence s owns q/o rows
  * [s*Lq,(s+1)*Lq) and k/v rows [s*Lk,(s+1)*Lk).  Non-causal, no mask.
  * Replaces F.scaled_dot_product_attention at iggt/layers/attention.py:61-66. */
@@ -269,7 +269,7 @@ int iggt_layernorm_rows(const float* x, int64_t ldx, int C, const float* w, cons
  * They exist so that tile selection, CTA pairing, stream-K and the attention work distribution are unit-tested. */
 
 /* Schedule of a GEMM launch. epi: 0 store16, 1 resid32, 2 qkv (N = 3C), 3 store32.
- * out[7] = {bn, pair (cta_group::2), stream_k, m_tiles (256-row pairs when pair), n_tiles, k_blocks, grid}. */
+ * out[7] = {bn, pair (always 0: no CTA pairs on sm_90), stream_k, m_tiles, n_tiles, k_blocks, grid}. */
 int iggt_gemm_plan(int epi, int M, int N, int K, int* out);
 
 /* Work items of CTA `cta` of a `grid`-CTA iggt_attention_fwd launch, in processing order, as quadruples

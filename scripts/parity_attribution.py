@@ -1,4 +1,4 @@
-"""CPU: where the end-to-end parity error of the B200 path comes from (no GPU needed; ~5 min on 16 threads).
+"""CPU: where the end-to-end parity error of the native path comes from (no GPU needed; ~5 min on 16 threads).
 
 The product's module graph is run with every C-ABI launcher replaced by its plain-PyTorch statement (tests/emu_ops.py,
 the same statements the GPU kernel tests hold the CUDA kernels to), with fp16 operands, against oracle/ref_model.py on a

@@ -1,4 +1,4 @@
-"""GPU: full-size parity report (BASELINE configs) of the B200 path against the oracle evaluated on the same GPU.
+"""GPU: full-size parity report (BASELINE configs) of the native path against the oracle evaluated on the same GPU.
 Writes gpurun_out/parity_fullsize.json (copied to profiles/ when judged).   python scripts/parity_fullsize.py [--quick]"""
 import argparse
 import json

@@ -1,4 +1,4 @@
-"""GPU: end-to-end parity report of the B200 path against the oracle (fp32 and same-precision-policy).
+"""GPU: end-to-end parity report of the native path against the oracle (fp32 and same-precision-policy).
 
 usage: python scripts/parity_report.py [--case NAME ...]   (cases = tests/golden fixtures + larger shapes)
 """

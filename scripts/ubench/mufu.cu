@@ -31,17 +31,18 @@ __global__ void k(float* out, int iters, float c) {
   out[blockIdx.x * blockDim.x + threadIdx.x] = acc;
 }
 int main() {
-  float* d; cudaMalloc(&d, 148 * 1024 * 4);
+  int sms; cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, 0);
+  float* d; cudaMalloc(&d, sms * 1024 * 4);
   cudaEvent_t e0, e1; cudaEventCreate(&e0); cudaEventCreate(&e1);
   int clk; cudaDeviceGetAttribute(&clk, cudaDevAttrClockRate, 0);
   for (int threads : {128, 256, 512, 1024}) for (int mode = 0; mode < 3; ++mode) {
     const int iters = 4096;
-    auto launch = [&]() { if (mode == 0) k<0><<<148, threads>>>(d, iters, 1.0001f); else if (mode == 1) k<1><<<148, threads>>>(d, iters, 1.0001f); else k<2><<<148, threads>>>(d, iters, 1.0001f); };
+    auto launch = [&]() { if (mode == 0) k<0><<<sms, threads>>>(d, iters, 1.0001f); else if (mode == 1) k<1><<<sms, threads>>>(d, iters, 1.0001f); else k<2><<<sms, threads>>>(d, iters, 1.0001f); };
     launch(); cudaDeviceSynchronize();
     cudaEventRecord(e0); launch(); cudaEventRecord(e1); cudaEventSynchronize(e1);
     float ms; cudaEventElapsedTime(&ms, e0, e1);
-    double exps = 148.0 * threads * iters * 16;
-    printf("threads %4d mode %d: %.3f ms  %.2f exp/ns/SM (at %.0f MHz nominal: %.2f exp/clk/SM)\n", threads, mode, ms, exps / (ms * 1e6) / 148, clk / 1e3, exps / (ms * 1e-3) / 148 / (clk * 1e3));
+    double exps = 1.0 * sms * threads * iters * 16;
+    printf("threads %4d mode %d: %.3f ms  %.2f exp/ns/SM (at %.0f MHz nominal: %.2f exp/clk/SM)\n", threads, mode, ms, exps / (ms * 1e6) / sms, clk / 1e3, exps / (ms * 1e-3) / sms / (clk * 1e3));
   }
   return 0;
 }

@@ -1,4 +1,4 @@
-"""TEST INFRASTRUCTURE (GPU): full-size parity of the B200 forward against oracle/ref_model.py evaluated on the same
+"""TEST INFRASTRUCTURE (GPU): full-size parity of the native forward against oracle/ref_model.py evaluated on the same
 device.  For one configuration `measure()` returns, per output key, the relative L2 / max distances
 
   vs_amp   product  vs  oracle(amp = trunk dtype, heads fp32)        <- the parity number

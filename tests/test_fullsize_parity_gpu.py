@@ -1,4 +1,4 @@
-"""GPU: parity of the B200 forward against the oracle AT THE BASELINE SIZES.  `oracle.ref_model.forward` is evaluated on
+"""GPU: parity of the native forward against the oracle AT THE BASELINE SIZES.  `oracle.ref_model.forward` is evaluated on
 the same GPU (exact-fp32 matmuls / convolutions, seconds per forward) with the trunk's autocast policy (`amp`) - the
 mode pinned against real autocast by tests/test_oracle_amp.py - and the product must agree with it on identical inputs.
 
@@ -12,10 +12,7 @@ Asserted, relative L2 against oracle(amp):
   fp16 trunk: depth, depth_conf, world_points_conf, pose_enc <= 1e-3 (north_star's figure);
               world_points, part_feat (amplified by sign*expm1 / 30+ conv layers; operands carry a 10-bit mantissa
               like the reference's own TF32 convolutions) <= 1.3 max(gap_amp, gap_tf32);
-  bf16 trunk: every key <= 1.2 x max(gap_amp, gap_tf32) (the heads still run fp16 operands, iggt/models/vggt.py:189).
-Measured on B200 (profiles/r02_parity_fullsize.json, stress weights): C2 fp16 depth 6.6e-4, conf 3.1e-4 / 4.8e-4,
-pose 5.1e-4, world_points 2.19e-3 = 1.09 x gap_tf32 (PyTorch's own TF32 heads sit 2.02e-3 from its fp32 heads on the
-same tokens); IGGT 8 x 532^2 part_feat 1.67e-3 = 1.18 x gap_tf32; bf16 trunks 0.3 - 0.7 x their gaps."""
+  bf16 trunk: every key <= 1.2 x max(gap_amp, gap_tf32) (the heads still run fp16 operands, iggt/models/vggt.py:189)."""
 import pytest
 import torch
 

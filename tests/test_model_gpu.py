@@ -2,7 +2,7 @@
 reference (fp32) and (b) the oracle under the same precision policy (fp16 trunk operands).
 
 Tolerances: the reference's own fp16-autocast vs fp32 gap on these weights is 4e-4 (depth) .. 1.3e-3
-(world_points) relative L2 (scripts/parity_report.py); the B200 path additionally keeps head activations in
+(world_points) relative L2 (scripts/parity_report.py); the native path additionally keeps head activations in
 16 bit, so it is asserted within 2e-3 (depth, conf) / 5e-3 (points, pose) relative L2 of the fp32 reference
 and within 5e-3 / 8e-3 element-wise relative to the tensor maximum."""
 import glob

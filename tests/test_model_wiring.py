@@ -1,4 +1,4 @@
-"""Host-side graph of the B200 model classes WITHOUT a GPU: every C-ABI launcher of `ops` is replaced by its plain
+"""Host-side graph of the native model classes WITHOUT a GPU: every C-ABI launcher of `ops` is replaced by its plain
 PyTorch statement (tests/emu_ops.py) and `VGGT.forward` must then reproduce the fixture of the unmodified reference.
 This pins what is NOT a kernel - weight packing, token / row layouts, the ResidualConvUnit and FeatureFusionBlock
 fusions of the DPT head (skip-adds and ReLUs folded into conv epilogues, 1x1 out_conv moved below the upsample),

@@ -1,5 +1,5 @@
 """The track-head oracle (SURVEY.md 8f row 4) against the fixture produced by the unmodified reference
-(`VGGT.forward(images, query_points)`, oracle/make_golden_track.py).  CPU only: this pins the restatement that the B200
+(`VGGT.forward(images, query_points)`, oracle/make_golden_track.py).  CPU only: this pins the restatement that the native
 track head (heads/track_head.py) is tested against in tests/test_track_wiring.py (CPU) and tests/test_track_gpu.py."""
 import os
 import sys

@@ -1,6 +1,6 @@
 """Host logic behind the launchers, exercised WITHOUT a GPU through the C ABI (`iggt_gemm_plan`,
-`iggt_attention_schedule`): N-tile choice, CTA pairing, stream-K, and the attention work distribution.  These are the
-decisions the C2 numbers in DESIGN.md rest on; the functions only run host code (148 SMs assumed without a device)."""
+`iggt_attention_schedule`): N-tile choice, stream-K, and the attention work distribution.  These are the decisions the
+C2 numbers in DESIGN.md rest on; the functions only run host code (an H100's 132 SMs assumed without a device)."""
 import ctypes
 
 import numpy as np
@@ -9,7 +9,7 @@ import pytest
 from iggt_official_b200 import _lib
 
 STORE16, RESID32, QKV, STORE32 = 0, 1, 2, 3
-SMS = 148
+SMS = 132
 
 
 def plan(epi, M, N, K):
@@ -28,15 +28,15 @@ def schedule(num_seq, Lq, Lk, H, grid, cta):
 def test_gemm_plan_c2_shapes():
     M = 8 * 1374                                            # the C2 token count
     qkv = plan(QKV, M, 3072, 1024)
-    assert (qkv["bn"], qkv["pair"], qkv["stream_k"]) == (256, 1, 0)
-    assert qkv["m_tiles"] == 43 and qkv["n_tiles"] == 12 and qkv["grid"] == SMS       # 74 CTA pairs
+    assert (qkv["bn"], qkv["pair"], qkv["stream_k"]) == (128, 0, 0)
+    assert qkv["m_tiles"] == 86 and qkv["n_tiles"] == 24 and qkv["grid"] == SMS
     fc1 = plan(STORE16, M, 4096, 1024)
-    assert (fc1["bn"], fc1["pair"], fc1["m_tiles"], fc1["n_tiles"], fc1["grid"]) == (256, 0, 86, 16, SMS)
-    for N, K in ((1024, 1024), (1024, 4096)):               # proj / fc2: 2.3 waves of pair tiles -> stream-K over pairs
+    assert (fc1["bn"], fc1["pair"], fc1["m_tiles"], fc1["n_tiles"], fc1["grid"]) == (128, 0, 86, 32, SMS)
+    for N, K in ((1024, 1024), (1024, 4096)):               # proj / fc2: 5.2 waves of 128 x 128 tiles -> stream-K
         r = plan(RESID32, M, N, K)
-        assert (r["bn"], r["pair"], r["stream_k"], r["grid"]) == (256, 1, 1, SMS)
-        assert r["m_tiles"] * r["n_tiles"] * r["k_blocks"] >= 4 * (SMS // 2)
-    cam = plan(RESID32, 8, 2048, 2048)                      # one row tile: nothing to pair, nothing to split
+        assert (r["bn"], r["pair"], r["stream_k"], r["grid"]) == (128, 0, 1, SMS)
+        assert r["m_tiles"] * r["n_tiles"] * r["k_blocks"] >= 4 * SMS
+    cam = plan(RESID32, 8, 2048, 2048)                      # one row tile: nothing to split
     assert cam["pair"] == 0 and cam["stream_k"] == 0 and cam["grid"] == cam["m_tiles"] * cam["n_tiles"]
 
 
@@ -48,15 +48,16 @@ def test_gemm_plan_invariants(epi):
         N = int(g.integers(1, 65)) * 64 if epi != QKV else 3 * 64 * int(g.integers(1, 33))
         K = int(g.integers(1, 129)) * 64
         p = plan(epi, M, N, K)
-        rows_per_tile = 256 if p["pair"] else 128
-        assert p["bn"] in (64, 128, 256) and (epi not in (RESID32, QKV) or p["bn"] >= 128)
+        rows_per_tile = 128
+        assert p["pair"] == 0
+        assert p["bn"] in (64, 128) and (epi not in (RESID32, QKV) or p["bn"] == 128)
         assert p["m_tiles"] * rows_per_tile >= M > (p["m_tiles"] - 1) * rows_per_tile      # rows covered, no spare tile
         assert p["n_tiles"] * p["bn"] >= N > (p["n_tiles"] - 1) * p["bn"]
         assert p["k_blocks"] * 64 >= K
-        assert 0 < p["grid"] <= SMS and (not p["pair"] or (p["bn"] == 256 and p["grid"] % 2 == 0))
-        assert not p["stream_k"] or (epi == RESID32 and p["bn"] == 256 and p["grid"] == SMS)
+        assert 0 < p["grid"] <= SMS
+        assert not p["stream_k"] or (epi == RESID32 and p["bn"] == 128 and p["grid"] == SMS)
         if not p["stream_k"]:
-            assert p["grid"] == min(p["m_tiles"] * p["n_tiles"], SMS // 2 if p["pair"] else SMS) * (2 if p["pair"] else 1)
+            assert p["grid"] == min(p["m_tiles"] * p["n_tiles"], SMS)
 
 
 def _check_attention(num_seq, Lq, H, grid):
@@ -81,14 +82,14 @@ def _check_attention(num_seq, Lq, H, grid):
 
 
 def test_attention_schedule_frame_shape_is_balanced():
-    """8 views x 16 heads x 1374 tokens: 640 full + 128 half items on 148 CTAs -> 5.0 item-times (round-robin: 6.0)."""
+    """8 views x 16 heads x 1374 tokens: 640 full + 128 half items on 132 CTAs -> 5.5 item-times (round-robin: 6.0)."""
     worst, mean = _check_attention(8, 1374, 16, SMS)
-    assert worst == 5.0 and abs(mean - 704 / SMS) < 1e-9
+    assert worst == 5.5 and abs(mean - 704 / SMS) < 1e-9
 
 
 def test_attention_schedule_global_shape_and_small_cases():
     worst, mean = _check_attention(1, 8 * 1374, 16, SMS)                # 86 tiles -> 43 full pairs, no light tail
-    assert worst == 5.0 and abs(mean - 688 / SMS) < 1e-9
+    assert worst == 6.0 and abs(mean - 688 / SMS) < 1e-9
     for num_seq, Lq, H in [(3, 300, 4), (1, 128, 1), (2, 129, 2), (1, 200, 2), (5, 1000, 3), (13, 405, 16), (1, 257, 1)]:
         total = num_seq * H * ((-(-Lq // 128) + 1) // 2)
         worst, mean = _check_attention(num_seq, Lq, H, min(total, SMS))
@@ -124,7 +125,7 @@ def test_attention_plan_splits_only_when_items_are_scarce():
     # one GPU, C2: plenty of items -> never split (the workspace traffic would cost more than the tail it balances)
     assert _plan(8, 1374, 1374, 16) == (1, 0)
     assert _plan(1, 8 * 1374, 8 * 1374, 16) == (1, 0)
-    # 8 GPUs, C2: 1 view per rank = 96 items for 148 SMs, 86 kv tiles each -> split the kv range
+    # 8 GPUs, C2: 1 view per rank = 96 items for 132 SMs, 86 kv tiles each -> split the kv range
     s, ws = _plan(1, 1374, 8 * 1374, 16)
     assert 3 <= s <= 8 and ws == s * 1374 * 16 * 66 * 4
     # 4 / 2 GPUs

@@ -1,4 +1,4 @@
-"""Host-side wiring of the B200 track head (heads/track_head.py) WITHOUT a GPU: the C-ABI launchers are replaced by
+"""Host-side wiring of the native track head (heads/track_head.py) WITHOUT a GPU: the C-ABI launchers are replaced by
 their plain-PyTorch statements (tests/emu_ops.py) and the module is driven teacher-forced against the fixture of the
 unmodified reference.  This pins row orders, the 48->64 head padding, the K / N zero padding, the separable positional
 embedding and the update-transformer plumbing; the CUDA kernels themselves are compared with the same statements in
