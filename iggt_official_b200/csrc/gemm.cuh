@@ -2,12 +2,17 @@
 //
 //   D[M,N] = epilogue( A[M,K] (16-bit, K-major) x W[N,K]^T (16-bit, K-major), fp32 accumulate in registers )
 //
-// One CTA per SM loops over 128 x BN output tiles (BN = 64 or 128). Warp roles: warp 0 = TMA producer (a ring of
-// 128B-swizzled A / W stages), warpgroups 1 and 2 = consumers: each issues the wgmma of 64 rows of the tile, then both
-// spill the fp32 accumulator to a shared-memory tile and act as two 4-warp epilogue groups (one row per thread,
-// 64-column chunks alternating between the groups: registers -> swizzled smem staging -> TMA store / TMA reduce-add).
-// The producer runs ahead into the next tile while the consumers work through an epilogue. Work is handed out by
-// WorkIter (whole tiles round-robin, or stream-K ranges of k-blocks for the residual epilogue).
+// One CTA per SM loops over 128 x BN output tiles (BN = 64 or 128). Work is handed out by WorkIter (whole tiles
+// round-robin, or stream-K ranges of k-blocks for the residual epilogue). Warp roles:
+//   warp 0       TMA producer: fills a ring of 128B-swizzled A / W stages in segment order (setmaxnreg: 40 registers)
+//   warpgroups 1 and 2: "ping-pong" consumers (setmaxnreg: 232 registers). Consumer warpgroup w owns segments w, w+2,
+//                w+4, ... of this CTA: it issues the wgmma of the whole 128 x BN tile (two m64 halves, BN fp32
+//                accumulator registers per thread), spills the accumulator to a shared fp32 tile and runs the epilogue
+//                (one row per thread: registers -> swizzled smem staging -> TMA store / TMA reduce-add, the two staging
+//                buffers alternating between column chunks).
+// Named barriers keep the two consumers in segment order, once for the main loops and once for the epilogues, so the
+// epilogue of segment s runs while the other warpgroup's main loop of segment s+1 keeps the tensor cores busy, and
+// one accumulator tile and one pair of staging buffers serve both warpgroups.
 //
 // Reference call sites this replaces (all via torch.nn on the reference side, SURVEY.md §2.2):
 //   qkv   iggt/layers/attention.py:52-58   (+ q/k LayerNorm(64) and 2-D RoPE, rope.py:154-188)
@@ -156,7 +161,10 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
                   const __grid_constant__ CUtensorMap tmC, const GemmParams p) {
   using SM = GemmSmem<BN>;
   constexpr int STAGES = SM::STAGES;
-  constexpr int G = 2;                                 // epilogue groups = consumer warpgroups
+  // named barriers: 1 + w = inside consumer warpgroup w; MMA_DONE + w = w has issued a segment's wgmma (the other
+  // warpgroup may start waiting on the next ring stages); EPI_DONE + w = w is through an epilogue (acc_tile, the
+  // per-column vectors and the staging buffers are free)
+  constexpr uint32_t BAR_MMA_DONE = 3, BAR_EPI_DONE = 5;
   extern __shared__ __align__(1024) uint8_t smem[];   // 128B-swizzled tiles need 1024-byte alignment
   if ((smem_u32(smem) & 1023u) != 0) __trap();
   uint8_t* smem_a = smem;
@@ -181,7 +189,7 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
   if (warp == 1 && lane == 0) {
     for (int i = 0; i < STAGES; ++i) {
       mbar_init(&full_bar[i], 1);
-      mbar_init(&empty_bar[i], G);                     // one arrival per consumer warpgroup
+      mbar_init(&empty_bar[i], 1);                     // each stage has one consumer warpgroup
     }
     fence_barrier_init();
   }
@@ -191,6 +199,7 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
 
   if (warp < 4) {
     // ------------------------------------------------------------ TMA producer
+    reg_dealloc<40>();
     if (warp == 0 && lane == 0) {
       int stage = 0;
       uint32_t phase = 0;
@@ -226,49 +235,68 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
     }
   } else {
     // ------------------------------------------------------------ consumers: main loop, then epilogue (1 row / thread)
-    const int grp = (warp - 4) >> 2;       // consumer warpgroup = epilogue group
-    const int ew = (warp - 4) & 3;         // warp inside the group
+    reg_alloc<232>();
+    const int wg = (warp - 4) >> 2;        // consumer warpgroup: owns segments wg, wg + 2, ...
+    const int ew = (warp - 4) & 3;         // warp inside the warpgroup
     const int row = ew * 32 + lane;        // epilogue: row inside the tile
     const bool leader = (ew == 0 && lane == 0);
-    constexpr int NBUF = 2 / G;            // staging buffers per group
-    uint8_t* const stg_grp = staging + grp * NBUF * SM::STG_BYTES;
-    const uint32_t bar_id = 1 + grp;
-    const int gtid = ew * 32 + lane;       // thread index inside the group
+    constexpr int NBUF = 2;                // staging buffers, alternating between the column chunks of a tile
+    const uint32_t bar_id = 1 + wg;
+    const int gtid = ew * 32 + lane;       // thread index inside the warpgroup
     float* const vb = epi_vec;                  // this tile's bias   [BN]
     float* const vg = vb + BN;                  // this tile's gamma  [BN]  (EPI_RESID32)
     float* const vn = vb + BN;                  // q_norm w,b | k_norm w,b  [4][64]  (EPI_QKV, BN >= 128)
     if constexpr (epi_is_qkv(EPI)) {
-      if (p.qk_norm) {
+      // written once; warpgroup 1 reads them only after warpgroup 0's first epilogue (BAR_EPI_DONE)
+      if (p.qk_norm && wg == 0) {
         for (int i = gtid; i < 64; i += 128) {
           vn[i] = p.qn_w[i]; vn[64 + i] = p.qn_b[i]; vn[128 + i] = p.kn_w[i]; vn[192 + i] = p.kn_b[i];
         }
       }
     }
-    int stage = 0;
-    uint32_t phase = 0;
     uint32_t store_count = 0;
     WorkIter work(p, worker, workers);
-    int tile, kb0, kb1;
-    while (work.next(tile, kb0, kb1)) {
+    int tile, kb0, kb1, ntile, nkb0, nkb1;
+    bool more = work.next(ntile, nkb0, nkb1);
+    uint32_t ring = 0;                     // ring position of the segment's first k-block
+    int seg_len = 0;
+    for (int seg = 0; more; ++seg) {
+      ring += seg_len;
+      tile = ntile; kb0 = nkb0; kb1 = nkb1;
+      seg_len = kb1 - kb0;
+      more = work.next(ntile, nkb0, nkb1);   // segment seg + 1 exists: its warpgroup waits for this segment's signals
+      if ((seg & 1) != wg) continue;
       const int mt = tile / p.num_n_tiles;
       const int nt = tile % p.num_n_tiles;
       const int n0 = nt * BN;
-      // ---- main loop: rows [64 grp, 64 grp + 64) of the tile
-      float acc[BN / 2];
+      // ---- main loop: the whole tile, rows [0, 64) into acc[0] and [64, 128) into acc[1].  It starts once segment
+      // seg - 1 has waited for all of its stages: the full barriers of the ring are then at most one phase ahead of
+      // this warpgroup's position, so the parity waits cannot alias.
+      if (seg > 0) named_bar_sync(BAR_MMA_DONE + (wg ^ 1), 256);
+      int stage = static_cast<int>(ring % STAGES);
+      uint32_t phase = (ring / STAGES) & 1;
+      float acc[2][BN / 2];
 #pragma unroll
-      for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+      for (int h = 0; h < 2; ++h) {
+#pragma unroll
+        for (int i = 0; i < BN / 2; ++i) acc[h][i] = 0.f;
+      }
       int prev_stage = -1;
       for (int kb = kb0; kb < kb1; ++kb) {
         mbar_wait(&full_bar[stage], phase);
-        const uint32_t a_addr = smem_u32(smem_a + stage * SM::A_BYTES) + grp * (64 * 128);
+        const uint32_t a_addr = smem_u32(smem_a + stage * SM::A_BYTES);
         const uint32_t b_addr = smem_u32(smem_b + stage * SM::B_BYTES);
         wgmma_fence();
 #pragma unroll
         for (int k = 0; k < GEMM_BK / 16; ++k) {
-          const uint64_t da = make_desc_sw128(a_addr + k * 32, 1024);
           const uint64_t db = make_desc_sw128(b_addr + k * 32, 1024);
-          if constexpr (BN == 128) wgmma_m64n128k16_ss<BF16>(acc, da, db, (kb != kb0 || k != 0) ? 1u : 0u);
-          else wgmma_m64n64k16_ss<BF16>(acc, da, db, (kb != kb0 || k != 0) ? 1u : 0u);
+          const uint32_t accumulate = (kb != kb0 || k != 0) ? 1u : 0u;
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            const uint64_t da = make_desc_sw128(a_addr + h * (64 * 128) + k * 32, 1024);
+            if constexpr (BN == 128) wgmma_m64n128k16_ss<BF16>(acc[h], da, db, accumulate);
+            else wgmma_m64n64k16_ss<BF16>(acc[h], da, db, accumulate);
+          }
         }
         wgmma_commit();
         // the previous k-block's MMAs have retired once at most this one is pending: free its smem slot
@@ -277,8 +305,10 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
         prev_stage = stage;
         if (++stage == STAGES) { stage = 0; phase ^= 1; }
       }
+      if (more) named_bar_arrive(BAR_MMA_DONE + wg, 256);   // the other warpgroup's main loop may start
       wgmma_wait<0>();
-      reg_fence(acc);
+      reg_fence(acc[0]);
+      reg_fence(acc[1]);
       if (prev_stage >= 0 && gtid == 0) mbar_arrive(&empty_bar[prev_stage]);
 
       int img = 0, y0 = 0, x0 = 0;
@@ -296,30 +326,31 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
         if (grow >= p.M) grow = -1;
       }
       // ---- accumulator fragments -> fp32 tile in smem (one row per epilogue thread from here on), per-column vectors
-      named_bar_sync(3, 128 * G);          // every epilogue thread is done with the previous tile's accumulator / vectors
-      {
-        const int r0 = grp * 64 + ew * 16 + (lane >> 2);
+      if (seg > 0) named_bar_sync(BAR_EPI_DONE + (wg ^ 1), 256);   // segment seg - 1's epilogue is done with them
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const int r0 = h * 64 + ew * 16 + (lane >> 2);
         float* const d0 = acc_tile + r0 * SM::ACC_LD + 2 * (lane & 3);
 #pragma unroll
         for (int j = 0; j < BN / 8; ++j) {
-          *reinterpret_cast<float2*>(d0 + 8 * j) = make_float2(acc[4 * j], acc[4 * j + 1]);
-          *reinterpret_cast<float2*>(d0 + 8 * SM::ACC_LD + 8 * j) = make_float2(acc[4 * j + 2], acc[4 * j + 3]);
+          *reinterpret_cast<float2*>(d0 + 8 * j) = make_float2(acc[h][4 * j], acc[h][4 * j + 1]);
+          *reinterpret_cast<float2*>(d0 + 8 * SM::ACC_LD + 8 * j) = make_float2(acc[h][4 * j + 2], acc[h][4 * j + 3]);
         }
       }
-      for (int i = grp * 128 + gtid; i < BN; i += 128 * G) {
+      for (int i = gtid; i < BN; i += 128) {
         const int col = n0 + i;
         vb[i] = (p.bias && col < p.N && kb0 == 0) ? __ldg(p.bias + col) : 0.f;   // bias rides with the first K segment
         if constexpr (EPI == EPI_RESID32) vg[i] = (p.gamma && col < p.N) ? __ldg(p.gamma + col) : 1.f;
       }
-      named_bar_sync(3, 128 * G);
+      named_bar_sync(bar_id, 128);
       const float* const t_row = acc_tile + row * SM::ACC_LD;
 
       if constexpr (EPI == EPI_STORE16 || epi_is_qkv(EPI)) {
         const int nvalid = min(BN / 64, (p.N - n0 + 63) / 64);
 #pragma unroll 1
-        for (int c64 = grp; c64 < nvalid; c64 += G) {
+        for (int c64 = 0; c64 < nvalid; ++c64) {
           const int col0 = n0 + c64 * 64;
-          uint8_t* stg = stg_grp + (store_count % NBUF) * SM::STG_BYTES;
+          uint8_t* stg = staging + (store_count % NBUF) * SM::STG_BYTES;
           if (leader) tma_store_wait_read<NBUF - 1>();
           named_bar_sync(bar_id, 128);
           float v[64];
@@ -479,9 +510,9 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
         // fp32 outputs: 32 columns (128 B) per staging tile
         const int nvalid = min(BN / 32, (p.N - n0 + 31) / 32);
 #pragma unroll 1
-        for (int c32 = grp; c32 < nvalid; c32 += G) {
+        for (int c32 = 0; c32 < nvalid; ++c32) {
           const int col0 = n0 + c32 * 32;
-          uint8_t* stg = stg_grp + (store_count % NBUF) * SM::STG_BYTES;
+          uint8_t* stg = staging + (store_count % NBUF) * SM::STG_BYTES;
           if (leader) tma_store_wait_read<NBUF - 1>();
           named_bar_sync(bar_id, 128);
           float v[32];
@@ -527,6 +558,8 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
           ++store_count;
         }
       }
+      if (leader) tma_store_wait_read<0>();   // the staging buffers are free for the other warpgroup's epilogue
+      if (more) named_bar_arrive(BAR_EPI_DONE + wg, 256);
     }
     if (leader) {
       tma_store_wait_all<0>();

@@ -6,8 +6,9 @@
 namespace iggt {
 
 // Pick the N tile: 128 wherever N allows it (a 128 x 128 tile reads 2 x 16 KB of operands per 64-deep k-block for
-// 2 x 64 x 128 x 64 MACs; the 64-wide tile needs the same A bytes for half the work).  Wider tiles do not fit: the
-// 64 x 256 fp32 accumulator of a consumer warpgroup would take all of its registers.
+// 2 x 64 x 128 x 64 MACs; the 64-wide tile needs the same A bytes for half the work).  Wider tiles do not fit: each
+// ping-pong consumer warpgroup holds the whole 128 x BN fp32 accumulator, BN registers per thread out of the 232 it
+// gets from setmaxnreg, and the epilogue needs its 64-value row chunk next to it; 128 x 256 would need 256.
 inline int choose_bn(int /*m_tiles*/, int N) { return N <= 64 ? 64 : 128; }
 
 // The host-side schedule of one GEMM launch, shared by the launchers and by iggt_gemm_plan (unit-tested without a GPU).

@@ -64,6 +64,23 @@ __device__ __forceinline__ void fence_proxy_async_smem() {
 __device__ __forceinline__ void named_bar_sync(uint32_t id, uint32_t nthreads) {
   asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
 }
+// signal a named barrier without waiting: the shared-memory writes before it are visible to the threads that bar.sync
+// on it (producer / consumer hand-off between warpgroups)
+__device__ __forceinline__ void named_bar_arrive(uint32_t id, uint32_t nthreads) {
+  asm volatile("bar.arrive %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
+}
+
+// ---------------------------------------------------------------- register reallocation between warpgroups
+// Executed by all four warps of a warpgroup: lower / raise the per-thread register limit of the warpgroup (a multiple
+// of 8 in [24, 256]); registers one warpgroup gives back can be taken by another of the same CTA.
+template <uint32_t N>
+__device__ __forceinline__ void reg_dealloc() {
+  asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N));
+}
+template <uint32_t N>
+__device__ __forceinline__ void reg_alloc() {
+  asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N));
+}
 
 // ---------------------------------------------------------------- TMA
 __device__ __forceinline__ void tma_prefetch_desc(const CUtensorMap* m) {
