@@ -72,6 +72,16 @@ SIGNATURES = {
     "iggt_knn_reorder": [c_void_p, c_void_p, c_int64, c_void_p, c_void_p, c_void_p],
     "iggt_knn_mean_features": [c_void_p, c_void_p, c_int64, c_int, c_void_p, c_int, c_void_p, c_void_p, c_void_p,
                                c_void_p, c_void_p],
+    "iggt_cluster_morton": [c_void_p, c_int64, c_void_p, c_void_p, c_void_p, c_void_p],
+    "iggt_cluster_reorder": [c_void_p, c_void_p, c_int64, c_void_p, c_void_p, c_void_p, c_void_p],
+    "iggt_cluster_core": [c_void_p, c_void_p, c_int64, c_int, c_void_p, c_void_p],
+    "iggt_cluster_mst_workspace": [c_int64, ctypes.POINTER(c_int64)],
+    "iggt_cluster_mst": [c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_void_p, c_void_p, c_void_p, c_void_p,
+                         ctypes.POINTER(ctypes.c_int32), c_void_p],
+    "iggt_cluster_fill": [c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_void_p, c_void_p, c_void_p, c_void_p,
+                          c_void_p],
+    "iggt_hdbscan_labels": [c_void_p, c_int64, c_int64, ctypes.c_double, c_void_p],
+    "iggt_mst_orient": [c_void_p, c_int64, c_int64],
     "iggt_avgpool2_nhwc": [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p],
     "iggt_sample_bilinear_nhwc": [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p],
     "iggt_corr_sample": [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int,

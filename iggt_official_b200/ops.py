@@ -498,6 +498,94 @@ def knn_mean_features(points, feats, k, return_graph=False, stats=None):
 
 
 # ---------------------------------------------------------------------------------------------------
+# HDBSCAN of the instance features (csrc/cluster.cu)
+def cluster_prepare(x):
+    """x [n,8] fp32 -> (sorted8 [n,8], orig [n] int32, box [ceil(n/256),16]): Morton order (stable library sort) and
+    the bounding box of every tile of 256 sorted points."""
+    assert x.is_cuda and x.dtype == torch.float32 and x.dim() == 2 and x.shape[1] == 8
+    x = x.contiguous()
+    n = x.shape[0]
+    assert 0 < n < 2 ** 31
+    lo, hi = x.amin(0).contiguous(), x.amax(0).contiguous()
+    codes = torch.empty(n, dtype=torch.int64, device=x.device)
+    _call(x, "iggt_cluster_morton", 0, 72.0 * n, x.data_ptr(), n, lo.data_ptr(), hi.data_ptr(), codes.data_ptr(), _STREAM)
+    order = torch.sort(codes, stable=True).indices
+    sorted8 = torch.empty_like(x)
+    orig = torch.empty(n, dtype=torch.int32, device=x.device)
+    box = torch.empty(((n + 255) // 256, 16), dtype=torch.float32, device=x.device)
+    _call(x, "iggt_cluster_reorder", 0, 76.0 * n, x.data_ptr(), order.data_ptr(), n, sorted8.data_ptr(), orig.data_ptr(),
+          box.data_ptr(), _STREAM)
+    return sorted8, orig, box
+
+
+def cluster_core(sorted8, box, k):
+    """Squared distance of every sorted point to its k-th nearest other point -> core2 [n] (sorted order)."""
+    n = sorted8.shape[0]
+    assert 1 <= k <= 512 and k < n
+    core2 = torch.empty(n, dtype=torch.float32, device=sorted8.device)
+    _call(sorted8, "iggt_cluster_core", 0, 36.0 * n, sorted8.data_ptr(), box.data_ptr(), n, int(k), core2.data_ptr(),
+          _STREAM)
+    return core2
+
+
+def cluster_mst(sorted8, box, orig, core2):
+    """Minimum spanning tree of the mutual-reachability graph -> (a [n-1] int32, b [n-1] int32, w2 [n-1] squared
+    weights, rounds): unsorted edges between original point indices."""
+    import ctypes
+    n = sorted8.shape[0]
+    assert n >= 2
+    ws_bytes = ctypes.c_int64()
+    _lib.check(_lib.load().iggt_cluster_mst_workspace(n, ctypes.byref(ws_bytes)), "iggt_cluster_mst_workspace")
+    ws = torch.empty(ws_bytes.value, dtype=torch.uint8, device=sorted8.device)
+    a = torch.empty(n - 1, dtype=torch.int32, device=sorted8.device)
+    b = torch.empty_like(a)
+    w2 = torch.empty(n - 1, dtype=torch.float32, device=sorted8.device)
+    rounds = ctypes.c_int32(0)
+    _call(sorted8, "iggt_cluster_mst", 0, 48.0 * n, sorted8.data_ptr(), box.data_ptr(), orig.data_ptr(), core2.data_ptr(),
+          n, ws.data_ptr(), a.data_ptr(), b.data_ptr(), w2.data_ptr(), ctypes.byref(rounds), _STREAM)
+    return a, b, w2, rounds.value
+
+
+def hdbscan_labels(mst, n, min_cluster_size, eps):
+    """Host (no GPU): mst [n-1,3] float64 (a, b, weight) sorted by weight -> labels [n] int64 (-1 = noise), numbered
+    as scikit-learn's tree_to_labels numbers them."""
+    import numpy as np
+    mst = np.ascontiguousarray(mst, dtype=np.float64)
+    assert mst.shape == (n - 1, 3)
+    labels = np.empty(n, dtype=np.int64)
+    _lib.check(_lib.load().iggt_hdbscan_labels(mst.ctypes.data, int(n), int(min_cluster_size), float(eps),
+                                               labels.ctypes.data), "iggt_hdbscan_labels")
+    return labels
+
+
+def mst_orient(mst, root=0):
+    """Host (no GPU): orients the rows (a, b, weight) of mst [n-1,3] float64 in place from parent to child of the tree
+    rooted at point `root` - the orientation scikit-learn's Prim MST from point 0 records."""
+    import numpy as np
+    assert isinstance(mst, np.ndarray) and mst.dtype == np.float64 and mst.flags.c_contiguous and mst.shape[1] == 3
+    _lib.check(_lib.load().iggt_mst_orient(mst.ctypes.data, mst.shape[0] + 1, int(root)), "iggt_mst_orient")
+    return mst
+
+
+def cluster_fill(sorted8, box, orig, label_sorted, palette=None):
+    """label_sorted [n] int32 (sorted order, -1 = noise, at least one labelled point) -> (labels [n] int64, rgb [n,3]
+    uint8 or None) at the original indices: noise points take the label of their nearest labelled point."""
+    n = sorted8.shape[0]
+    assert label_sorted.dtype == torch.int32 and label_sorted.shape == (n,)
+    dev = sorted8.device
+    tile_count = torch.empty((n + 255) // 256, dtype=torch.int32, device=dev)
+    out = torch.empty(n, dtype=torch.int64, device=dev)
+    rgb = None
+    if palette is not None:
+        assert palette.dtype == torch.uint8 and palette.is_cuda and palette.dim() == 2 and palette.shape[1] == 3
+        palette = palette.contiguous()
+        rgb = torch.empty((n, 3), dtype=torch.uint8, device=dev)
+    _call(sorted8, "iggt_cluster_fill", 0, 48.0 * n, sorted8.data_ptr(), box.data_ptr(), orig.data_ptr(),
+          label_sorted.data_ptr(), n, tile_count.data_ptr(), _ptr(palette), out.data_ptr(), _ptr(rgb), _STREAM)
+    return out, rgb
+
+
+# ---------------------------------------------------------------------------------------------------
 # Track head (csrc/track.cu)
 def avgpool2_nhwc(x):
     """[NB,H,W,C] 16-bit -> [NB,H//2,W//2,C]."""

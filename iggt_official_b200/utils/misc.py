@@ -1,9 +1,14 @@
-"""Device-side instance-clustering front-end (SURVEY.md section 8f, row 2).
+"""Device-side instance clustering (SURVEY.md section 8f, row 2): the last step of the demo (demo.py:365-401).
 
 `knn_avg_features_pyg` keeps the name and arguments of the reference helper (iggt/utils/misc.py:24-78), which builds
 a k-NN graph over the un-projected points of ALL views with torch_geometric and averages the neighbours' features with
-torch_scatter on the CPU; here it is one exact block-pruned search on the GPU (csrc/knn.cu).  HDBSCAN itself stays a
-third-party library on the reference side as well (cuML / hdbscan) and is out of scope."""
+torch_scatter on the CPU; here it is one exact block-pruned search on the GPU (csrc/knn.cu).
+
+`cluster_features_to_masks_mv` keeps the name, arguments and return values of the reference helper
+(iggt/utils/misc.py:81-170), which runs cuML's or the contrib `hdbscan` package's HDBSCAN over all pixels on the host.
+Here the core distances, the minimum spanning tree of the mutual-reachability graph and the noise fill run on the GPU
+(csrc/cluster.cu); only the tree condensation and cluster selection, O(n) work over the MST edges, run on the host
+inside the same library."""
 import numpy as np
 import torch
 
@@ -24,3 +29,105 @@ def knn_avg_features_pyg(points_batch, features_batch, k, device="cuda"):
     N, H, W, F = features_batch.shape
     out = ops.knn_mean_features(points_batch.reshape(-1, 3), features_batch.reshape(-1, F), int(k))
     return out.view(N, H, W, F)
+
+
+# matplotlib's `jet` segment data, per channel (x, y0, y1).  The table below restates matplotlib's lookup-table
+# construction from this public data; matplotlib is not a dependency, and the table has not been checked against a
+# matplotlib install.
+_JET_SEGMENTS = (
+    ((0.0, 0.0, 0.0), (0.35, 0.0, 0.0), (0.66, 1.0, 1.0), (0.89, 1.0, 1.0), (1.0, 0.5, 0.5)),
+    ((0.0, 0.0, 0.0), (0.125, 0.0, 0.0), (0.375, 1.0, 1.0), (0.64, 1.0, 1.0), (0.91, 0.0, 0.0), (1.0, 0.0, 0.0)),
+    ((0.0, 0.5, 0.5), (0.11, 1.0, 1.0), (0.34, 1.0, 1.0), (0.65, 0.0, 0.0), (1.0, 0.0, 0.0)),
+)
+
+
+def jet_lut(n=256):
+    """[n, 3] float64: `jet` sampled at n evenly spaced points of [0, 1], piecewise linear between the segment rows."""
+    out = []
+    for seg in _JET_SEGMENTS:
+        a = np.asarray(seg, np.float64)
+        x, y0, y1 = a[:, 0] * (n - 1), a[:, 1], a[:, 2]
+        xs = (n - 1) * np.linspace(0.0, 1.0, n)
+        ind = np.searchsorted(x, xs)[1:-1]
+        frac = (xs[1:-1] - x[ind - 1]) / (x[ind] - x[ind - 1])
+        out.append(np.clip(np.concatenate([[y1[0]], frac * (y0[ind] - y1[ind - 1]) + y1[ind - 1], [y0[-1]]]), 0, 1))
+    return np.stack(out, 1)
+
+
+def label_palette(labels):
+    """uint8 [max label + 1, 3]: the reference's colours, sorted label j -> jet(j / (k - 1)) (jet(0.5) if k == 1),
+    truncated by (rgb * 255).astype(uint8).  `labels` holds the distinct non-negative labels."""
+    uniq = np.unique(labels)
+    lut = jet_lut()
+    k = len(uniq)
+    pal = np.zeros((int(uniq[-1]) + 1, 3), np.uint8)
+    for j, lab in enumerate(uniq):
+        x = j / (k - 1) if k > 1 else 0.5
+        pal[lab] = (lut[min(int(x * 256), 255)] * 255).astype(np.uint8)
+    return pal
+
+
+def sorted_mst(a, b, w2):
+    """Device MST edges -> [n-1, 3] float64 (a, b, weight) rows on the host, sorted by (weight, smaller index,
+    larger index) so that equal weights keep a fixed order, each edge oriented from the side of point 0 as
+    scikit-learn's Prim MST records it (which side is left in the single-linkage tree decides the cluster numbers)."""
+    lo, hi = torch.minimum(a, b), torch.maximum(a, b)
+    i = torch.argsort(hi, stable=True)
+    i = i[torch.argsort(lo[i], stable=True)]
+    i = i[torch.argsort(w2[i], stable=True)]
+    mst = torch.stack([a[i].double(), b[i].double(), torch.sqrt(w2[i].double())], 1).cpu().numpy()
+    return ops.mst_orient(np.ascontiguousarray(mst))
+
+
+def hdbscan_device(x, eps, min_samples, min_cluster_size):
+    """x [n, 8] fp32 CUDA -> (raw labels [n] int64 ndarray, -1 = noise; (sorted8, orig, box) of the tile search)."""
+    sorted8, orig, box = ops.cluster_prepare(x)
+    core2 = ops.cluster_core(sorted8, box, min_samples)
+    a, b, w2, _ = ops.cluster_mst(sorted8, box, orig, core2)
+    raw = ops.hdbscan_labels(sorted_mst(a, b, w2), x.shape[0], min_cluster_size, eps)
+    return raw, (sorted8, orig, box)
+
+
+def cluster_features_to_masks_mv(feature_map, apply_colormap=False, **kwargs):
+    """HDBSCAN over the pixels of all views together, with the contrib `hdbscan` package's semantics (Euclidean,
+    min_samples = neighbours besides the point itself, excess of mass, cluster_selection_epsilon = eps, no single
+    cluster); noise pixels then take the label of their nearest labelled pixel in feature space (ties: lowest pixel
+    index), and all labels become 0 if every pixel is noise.
+
+    feature_map [N, H, W, C] (C <= 8; tensor or ndarray; CUDA tensors are used in place) and the keyword arguments
+    eps, min_samples (<= 512) and min_cluster_size (>= 2); others (e.g. method="dbscan") are ignored.
+    Returns masks [N, H, W] int64, and with apply_colormap also colours [N, H, W, 3] uint8, as ndarrays."""
+    if not (isinstance(feature_map, (torch.Tensor, np.ndarray)) and feature_map.ndim == 4):
+        raise ValueError("feature_map must be a 4-D [N, H, W, C] tensor or ndarray")
+    eps, min_samples, min_cluster_size = (kwargs.get(k) for k in ("eps", "min_samples", "min_cluster_size"))
+    if eps is None or min_samples is None or min_cluster_size is None:
+        raise ValueError("cluster_features_to_masks_mv needs eps, min_samples and min_cluster_size")
+    eps, min_samples, min_cluster_size = float(eps), int(min_samples), int(min_cluster_size)
+    if not (np.isfinite(eps) and eps >= 0 and 1 <= min_samples <= 512 and min_cluster_size >= 2):
+        raise ValueError(f"unsupported eps={eps}, min_samples={min_samples}, min_cluster_size={min_cluster_size}")
+    N, H, W, C = feature_map.shape
+    if not 1 <= C <= 8:
+        raise ValueError(f"feature_map has {C} channels; 1 to 8 are supported")
+    n = N * H * W
+    if n < min_samples + 1:
+        raise ValueError(f"{n} points: HDBSCAN with min_samples={min_samples} needs at least {min_samples + 1}")
+    x = torch.as_tensor(feature_map)
+    if not x.is_cuda:
+        if not torch.cuda.is_available():
+            raise RuntimeError("iggt_official_b200 has no CPU path: cluster_features_to_masks_mv needs a CUDA device")
+        x = x.cuda()
+    with torch.cuda.device(x.device):
+        x = x.reshape(n, C).to(torch.float32)
+        if not bool(torch.isfinite(x).all()):
+            raise ValueError("feature_map has non-finite values")
+        x = torch.nn.functional.pad(x, (0, 8 - C)).contiguous()     # zero channels leave the distances unchanged
+        raw, (sorted8, orig, box) = hdbscan_device(x, eps, min_samples, min_cluster_size)
+        if (raw < 0).all():
+            raw = np.zeros_like(raw)
+        label_sorted = torch.from_numpy(raw.astype(np.int32)).to(x.device)[orig.long()]
+        palette = torch.from_numpy(label_palette(raw[raw >= 0])).to(x.device) if apply_colormap else None
+        labels, rgb = ops.cluster_fill(sorted8, box, orig, label_sorted, palette)
+        masks = labels.view(N, H, W).cpu().numpy()
+        if not apply_colormap:
+            return masks
+        return masks, rgb.view(N, H, W, 3).cpu().numpy()

@@ -311,6 +311,51 @@ int iggt_knn_reorder(const float* points, const int64_t* order, int64_t n, float
 int iggt_knn_mean_features(const float* sorted4, const float* aabb, int64_t n, int k, const float* feats, int F,
                            float* out, int32_t* out_idx, float* out_d2, uint64_t* stats, iggt_stream_t stream);
 
+/* ---- HDBSCAN of the instance features (iggt/utils/misc.py:81-170: cluster_features_to_masks_mv, contrib `hdbscan`
+ * semantics).  8-d fp32 points; Morton-ordered tiles of 256 points with 8-d boxes, exact block-pruned searches
+ * (csrc/cluster.cu).  Distances are squared throughout. */
+
+/* 56-bit Morton key of every point feats8 [n,8] on a 128^8 lattice over the per-axis extent lo[8]..hi[8]. */
+int iggt_cluster_morton(const float* feats8, int64_t n, const float* lo, const float* hi, int64_t* codes,
+                        iggt_stream_t stream);
+
+/* order[n] (a permutation) -> sorted8 [n,8], orig [n] (original index of each sorted point) and
+ * box [ceil(n/256), 16] = (min 8, max 8) of every tile of 256 consecutive sorted points. */
+int iggt_cluster_reorder(const float* feats8, const int64_t* order, int64_t n, float* sorted8, int32_t* orig,
+                         float* box, iggt_stream_t stream);
+
+/* core2 [n] (sorted order): squared distance of every point to its k-th nearest OTHER point, 1 <= k <= 512, k < n. */
+int iggt_cluster_core(const float* sorted8, const float* box, int64_t n, int k, float* core2, iggt_stream_t stream);
+
+/* Host query: *bytes = device workspace size of iggt_cluster_mst for n points. */
+int iggt_cluster_mst_workspace(int64_t n, int64_t* bytes);
+
+/* Minimum spanning tree of the mutual-reachability graph max(core_i, core_j, d_ij) by Boruvka (ties: lower weight,
+ * then smaller, then larger original index).  Writes n-1 unsorted edges edge_a/edge_b (original indices, edge_a is
+ * the endpoint in the component that picked the edge) and edge_w2 (squared weights); *rounds (host pointer, may be
+ * NULL) = Boruvka rounds.  Synchronises the stream once per pointer-jumping pass.  -2 / -3: no spanning tree was found. */
+int iggt_cluster_mst(const float* sorted8, const float* box, const int32_t* orig, const float* core2, int64_t n,
+                     void* workspace, int32_t* edge_a, int32_t* edge_b, float* edge_w2, int32_t* rounds,
+                     iggt_stream_t stream);
+
+/* Noise fill: label [n] (sorted order, -1 = noise; at least one labelled point) -> out_label [n] int64 at the original
+ * index, a noise point taking the label of its nearest labelled point (ties: lowest original index).  With out_rgb
+ * [n,3] (may be NULL), also palette[label] (uint8 [labels,3]).  tile_count: workspace of ceil(n/256) ints. */
+int iggt_cluster_fill(const float* sorted8, const float* box, const int32_t* orig, const int32_t* label, int64_t n,
+                      int32_t* tile_count, const uint8_t* palette, int64_t* out_label, uint8_t* out_rgb,
+                      iggt_stream_t stream);
+
+/* HOST function (no GPU): orients every edge of mst [n-1,3] (a, b, weight) in place from parent to child of the tree
+ * rooted at point `root`.  scikit-learn builds its MST with Prim's algorithm from point 0, which records every edge
+ * from the tree side, and the single-linkage tree puts the first endpoint's side on the left: with root 0, the cluster
+ * numbering of iggt_hdbscan_labels then follows scikit-learn's for the same tree.  -2: not a spanning tree. */
+int iggt_mst_orient(double* mst, int64_t n, int64_t root);
+
+/* HOST function (no GPU): labels [n] (-1 = noise) from an MST given as mst [n-1,3] = (a, b, weight) rows in float64,
+ * sorted by weight, exactly as scikit-learn 1.9's tree_to_labels(make_single_linkage(mst), min_cluster_size, "eom",
+ * allow_single_cluster=False, cluster_selection_epsilon=eps).  -2: the edges do not form a spanning tree. */
+int iggt_hdbscan_labels(const double* mst, int64_t n, int64_t min_cluster_size, double eps, int64_t* labels);
+
 #ifdef __cplusplus
 }
 #endif
