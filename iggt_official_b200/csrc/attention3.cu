@@ -178,13 +178,12 @@ attention3_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant
         const bool has_next = items.peek(nqp, nhead, nseq, nb);
         const int col = head * A3_D;
         for (int j = j0; j < j1; ++j) {
-          const int row = seq * p.Lk + j * A3_BK;
           mbar_wait(&k_empty[st], ph ^ 1);
           mbar_expect_tx(&k_full[st], A3_TILE);
-          tma_load_2d(sK + st * A3_TILE, &tmK, &k_full[st], col, row);
+          tma_load_3d(sK + st * A3_TILE, &tmK, &k_full[st], col, j * A3_BK, seq);
           mbar_wait(&v_empty[st], ph ^ 1);
           mbar_expect_tx(&v_full[st], A3_TILE);
-          tma_load_2d(sV + st * A3_TILE, &tmV, &v_full[st], col, row);
+          tma_load_3d(sV + st * A3_TILE, &tmV, &v_full[st], col, j * A3_BK, seq);
           if (++st == A3_STAGES) { st = 0; ph ^= 1; }
           if (j == j0 && has_next) load_q(nqp, nhead, nseq, nb);
         }
@@ -511,8 +510,17 @@ int attention_launch(const void* q, int64_t ldq, const void* k, int64_t ldk, con
   const TmDtype dt = dtype ? TM_BF16 : TM_F16;
   CUtensorMap tQ, tK, tV;
   if (make_tmap_2d(&tQ, dt, q, (uint64_t)num_seq * Lq, (uint64_t)H * 64, ldq, 64, A3_BQ)) return -4;
-  if (make_tmap_2d(&tK, dt, k, (uint64_t)num_seq * Lk, (uint64_t)H * 64, ldk, 64, A3_BK)) return -4;
-  if (make_tmap_2d(&tV, dt, v, (uint64_t)num_seq * Lk, (uint64_t)H * 64, ldv, 64, A3_BK)) return -4;
+  // K and V are 3-D {H*64 columns, Lk rows, num_seq sequences}: the ragged last key tile of a sequence reads zeros past
+  // row Lk (TMA fill), never the next sequence's rows.  The mask gives those keys P = 0, but 0 * V is NaN where V is inf,
+  // so with a 2-D map over all sequences one sequence's output could depend on its neighbour's values.
+  {
+    const uint64_t dims[3] = {(uint64_t)H * 64, (uint64_t)Lk, (uint64_t)num_seq};
+    const uint32_t box[3] = {64, A3_BK, 1};
+    const uint64_t kstr[2] = {(uint64_t)ldk * 2, (uint64_t)Lk * ldk * 2};
+    const uint64_t vstr[2] = {(uint64_t)ldv * 2, (uint64_t)Lk * ldv * 2};
+    if (make_tmap(&tK, dt, 3, k, dims, kstr, box)) return -4;
+    if (make_tmap(&tV, dt, 3, v, dims, vstr, box)) return -4;
+  }
   Attn3Params p;
   attn3_shape(p, num_seq, Lq, Lk, H, splits);
   const int n_kv = (Lk + A3_BK - 1) / A3_BK;
