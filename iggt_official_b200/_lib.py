@@ -82,6 +82,15 @@ SIGNATURES = {
                           c_void_p],
     "iggt_hdbscan_labels": [c_void_p, c_int64, c_int64, ctypes.c_double, c_void_p],
     "iggt_mst_orient": [c_void_p, c_int64, c_int64],
+    "iggt_pca_basis_workspace": [c_int, ctypes.POINTER(c_int64)],
+    "iggt_pca_basis": [c_void_p, c_int64, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
+                       c_void_p],
+    "iggt_pca_project": [c_void_p, c_int64, c_int, c_void_p, c_void_p, c_int64, c_void_p],
+    "iggt_quantile_workspace": [c_int64, ctypes.POINTER(c_int64)],
+    "iggt_quantile": [c_void_p, c_int64, c_int64, c_int64, ctypes.POINTER(c_float), c_int, c_void_p, c_void_p,
+                      c_void_p],
+    "iggt_pca_stretch": [c_void_p, c_int64, c_int64, c_void_p, c_void_p, c_void_p],
+    "iggt_sym_eig": [c_void_p, c_int, c_void_p, c_void_p],
     "iggt_avgpool2_nhwc": [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p],
     "iggt_sample_bilinear_nhwc": [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p],
     "iggt_corr_sample": [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int,

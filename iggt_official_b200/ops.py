@@ -586,6 +586,100 @@ def cluster_fill(sorted8, box, orig, label_sorted, palette=None):
 
 
 # ---------------------------------------------------------------------------------------------------
+# PCA feature colours and exact quantiles (csrc/pca.cu)
+class PcaBasis:
+    """Device outputs of iggt_pca_basis: moments [C + C(C+1)/2] f64, cov [C,C] f64, evals [C] f64, evecs [C,C] f64,
+    V [C,3] fp32 (the first three eigenvectors) and nonfinite [1] int64."""
+
+    def __init__(self, C, device):
+        f64 = dict(dtype=torch.float64, device=device)
+        self.moments = torch.empty(C + C * (C + 1) // 2, **f64)
+        self.cov = torch.empty((C, C), **f64)
+        self.evals = torch.empty(C, **f64)
+        self.evecs = torch.empty((C, C), **f64)
+        self.V = torch.empty((C, 3), dtype=torch.float32, device=device)
+        self.nonfinite = torch.empty(1, dtype=torch.int64, device=device)
+
+
+def _workspace(query, *args):
+    import ctypes
+    nbytes = ctypes.c_int64()
+    _lib.check(getattr(_lib.load(), query)(*args, ctypes.byref(nbytes)), query)
+    return nbytes.value
+
+
+def pca_basis(x):
+    """x [n,C] fp32 (3 <= C <= 8) -> PcaBasis: fixed-order fp64 moments, the sample covariance and its Jacobi
+    eigendecomposition, all on the device (no host synchronisation)."""
+    assert x.is_cuda and x.dtype == torch.float32 and x.dim() == 2 and 3 <= x.shape[1] <= 8
+    x = x.contiguous()
+    n, C = x.shape
+    assert n > 0
+    ws = torch.empty(_workspace("iggt_pca_basis_workspace", C), dtype=torch.uint8, device=x.device)
+    b = PcaBasis(C, x.device)
+    _call(x, "iggt_pca_basis", 3.0 * n * C * (C + 3), 4.0 * n * C, x.data_ptr(), n, C, ws.data_ptr(), b.moments.data_ptr(),
+          b.cov.data_ptr(), b.evals.data_ptr(), b.evecs.data_ptr(), b.V.data_ptr(), b.nonfinite.data_ptr(), _STREAM)
+    return b
+
+
+def pca_project(x, V):
+    """x [n,C] fp32, V [C,3] fp32 -> y [3,n] fp32 = (x @ V).T (fp32 fmas in channel order).  The rows of y are
+    padded to a multiple of 4 floats (16-byte aligned rows for the later stages)."""
+    assert x.is_cuda and x.dtype == torch.float32 and x.dim() == 2 and 3 <= x.shape[1] <= 8
+    x = x.contiguous()
+    n, C = x.shape
+    assert V.dtype == torch.float32 and V.shape == (C, 3)
+    V = V.contiguous()
+    ldy = (n + 3) // 4 * 4
+    y = torch.empty((3, ldy), dtype=torch.float32, device=x.device)
+    _call(x, "iggt_pca_project", 6.0 * n * C, 4.0 * n * (C + 3), x.data_ptr(), n, C, V.data_ptr(), y.data_ptr(), ldy,
+          _STREAM)
+    return y[:, :n]
+
+
+def quantile(y, q):
+    """y [rows,n] fp32 (unit column stride), q: sequence of floats in [0, 1] -> [rows, len(q)] fp32, equal to
+    torch.quantile(y[r], q[i]) bit for bit (linear interpolation; a row with a NaN gives NaN), for any n < 2^32."""
+    import ctypes
+    assert y.is_cuda and y.dtype == torch.float32 and y.dim() == 2 and y.stride(1) == 1
+    rows, n = y.shape
+    q = [float(v) for v in q]
+    assert 0 < rows <= 65535 and 0 < n < 2 ** 32 and len(q) > 0 and all(0.0 <= v <= 1.0 for v in q)
+    ws = torch.empty(_workspace("iggt_quantile_workspace", rows), dtype=torch.uint8, device=y.device)
+    out = torch.empty((rows, len(q)), dtype=torch.float32, device=y.device)
+    qa = (ctypes.c_float * len(q))(*q)
+    passes = 3 * ((len(q) + 1) // 2)                      # three radix passes per pair of quantiles
+    _call(y, "iggt_quantile", 0, 4.0 * rows * n * passes, y.data_ptr(), rows, n, y.stride(0), qa, len(q), ws.data_ptr(),
+          out.data_ptr(), _STREAM)
+    return out
+
+
+def pca_stretch(y, qv):
+    """y [3,n] fp32 (unit column stride), qv [3,2] fp32 (lo, hi) -> out [n,3] fp32 =
+    clamp((y.T - lo) / (hi - lo), 0, 1), 0.5 in a channel whose hi <= lo."""
+    assert y.is_cuda and y.dtype == torch.float32 and y.dim() == 2 and y.shape[0] == 3 and y.stride(1) == 1
+    assert qv.is_cuda and qv.dtype == torch.float32 and qv.shape == (3, 2)
+    qv = qv.contiguous()
+    n = y.shape[1]
+    out = torch.empty((n, 3), dtype=torch.float32, device=y.device)
+    _call(y, "iggt_pca_stretch", 3.0 * n, 24.0 * n, y.data_ptr(), n, y.stride(0), qv.data_ptr(), out.data_ptr(), _STREAM)
+    return out
+
+
+def sym_eig(a):
+    """Host (no GPU): a [C,C] float64 symmetric (1 <= C <= 8) -> (evals [C] descending, evecs [C,C] with eigenvector j
+    in column j, its largest-magnitude component positive) by the cyclic Jacobi code iggt_pca_basis runs."""
+    import numpy as np
+    a = np.ascontiguousarray(a, dtype=np.float64)
+    C = a.shape[0]
+    assert a.shape == (C, C) and 1 <= C <= 8
+    evals = np.empty(C, np.float64)
+    evecs = np.empty((C, C), np.float64)
+    _lib.check(_lib.load().iggt_sym_eig(a.ctypes.data, C, evals.ctypes.data, evecs.ctypes.data), "iggt_sym_eig")
+    return evals, evecs
+
+
+# ---------------------------------------------------------------------------------------------------
 # Track head (csrc/track.cu)
 def avgpool2_nhwc(x):
     """[NB,H,W,C] 16-bit -> [NB,H//2,W//2,C]."""

@@ -356,6 +356,42 @@ int iggt_mst_orient(double* mst, int64_t n, int64_t root);
  * allow_single_cluster=False, cluster_selection_epsilon=eps).  -2: the edges do not form a spanning tree. */
 int iggt_hdbscan_labels(const double* mst, int64_t n, int64_t min_cluster_size, double eps, int64_t* labels);
 
+/* ---- PCA feature colours (iggt/utils/misc.py:272-332: apply_pca_colormap, torch.pca_lowrank + torch.quantile) and
+ * exact quantiles (csrc/pca.cu).  x [n, C] fp32, 3 <= C <= 8. */
+
+/* Host query: *bytes = device workspace size of iggt_pca_basis for C channels. */
+int iggt_pca_basis_workspace(int C, int64_t* bytes);
+
+/* One pass over x: moments [C + C(C+1)/2] fp64 = sums of d = x - x[0] and of d d^T (upper triangle, row-major) and
+ * *nonfinite = number of non-finite values, reduced in a fixed order (bit-identical on repeated calls on one device);
+ * then one CTA forms cov [C, C] = the sample covariance (all 0 if nonfinite > 0), decomposes it as iggt_sym_eig does
+ * (evals [C], evecs [C, C]) and writes V [C, 3] fp32 = the first three eigenvectors. */
+int iggt_pca_basis(const float* x, int64_t n, int C, void* workspace, double* moments, double* cov, double* evals,
+                   double* evecs, float* V, int64_t* nonfinite, iggt_stream_t stream);
+
+/* y [3, n] (row pitch ldy) = (x V)^T: y[j, i] = sum_c x[i, c] V[c, j], fp32 fmas in channel order. */
+int iggt_pca_project(const float* x, int64_t n, int C, const float* V, float* y, int64_t ldy, iggt_stream_t stream);
+
+/* Host query: *bytes = device workspace size of iggt_quantile for `rows` rows (<= 65535). */
+int iggt_quantile_workspace(int64_t rows, int64_t* bytes);
+
+/* out [rows, nq] fp32 = torch.quantile(y[r, :n], q[i]) (linear interpolation), bit for bit, for every row r of
+ * y [rows, n] (row pitch ld) and every q[i] in [0, 1] (q is a HOST array).  The rank is float32(q) * float32(n - 1)
+ * (clamped to n - 1); the floor and ceil order statistics come from a radix selection, no sort, any n < 2^32.
+ * A row holding a NaN gives NaN. */
+int iggt_quantile(const float* y, int64_t rows, int64_t n, int64_t ld, const float* q, int nq, void* workspace,
+                  float* out, iggt_stream_t stream);
+
+/* out [n, 3] = clamp((y[j, i] - lo_j) / (hi_j - lo_j), 0, 1), or 0.5 where hi_j <= lo_j, for y [3, n] (row pitch ldy)
+ * and qv [3, 2] = (lo_j, hi_j) (device pointer, e.g. iggt_quantile's output for q = 0.02, 0.98). */
+int iggt_pca_stretch(const float* y, int64_t n, int64_t ldy, const float* qv, float* out, iggt_stream_t stream);
+
+/* HOST function (no GPU): symmetric eigendecomposition of a [C, C] (row-major fp64, upper triangle read, 1 <= C <= 8)
+ * by cyclic Jacobi, the same code iggt_pca_basis runs on the device.  evals [C] descending (ties: lower index first);
+ * evecs [C, C] row-major with eigenvector j in column j, its largest-magnitude component positive (the first one
+ * when several tie).  -1: a non-finite entry. */
+int iggt_sym_eig(const double* a, int C, double* evals, double* evecs);
+
 #ifdef __cplusplus
 }
 #endif
