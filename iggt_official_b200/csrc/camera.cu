@@ -541,6 +541,14 @@ extern "C" int iggt_camera_head(const iggt_camera_weights* w, const float* token
 
   const int sms = device_sm_count();
   const int grid = sms >= 128 ? 128 : sms;           // 128 | every tile count of the head (128 / 384 / 512): no ragged wave
+  // the consumers keep at most 4 tiles of a phase in registers (acc[4]) while the producer streams the stages of every
+  // tile it assigns to the CTA: below 128 SMs (fc1: 512 tiles) a CTA would own 5 and the weight ring would fall out of
+  // step, so such devices take the per-layer launches
+  int max_tiles = 0;
+  for (int i = 0; i < np; ++i)
+    if (prog.ph[i].type == PH_GEMM && (prog.ph[i].N + CAM_COLS - 1) / CAM_COLS > max_tiles)
+      max_tiles = (prog.ph[i].N + CAM_COLS - 1) / CAM_COLS;
+  if ((max_tiles + grid - 1) / grid > 4) return -7;
   void (*kern)(const CamProgram) = nullptr;
   if (prog.Mpad == 8) kern = dtype ? camera_head_kernel<true, 8> : camera_head_kernel<false, 8>;
   else kern = dtype ? camera_head_kernel<true, 16> : camera_head_kernel<false, 16>;

@@ -4,8 +4,9 @@
 M = B*S rows of width 2048 against 216 M parameters: every Linear is a weight stream (fp32 activations, 16-bit
 weights, fp32 accumulate).  For B*S <= 16 the whole head - 4 iterations x (embed, AdaLN, 4 blocks, pose branch) - is ONE
 persistent launch (`iggt_camera_head`, csrc/camera.cu: the producer warp streams weights across phase boundaries, a
-device-wide barrier separates the ~27 phases of an iteration).  Larger batches (and IGGT_CAMERA_FUSED=0) run layer by
-layer: `iggt_skinny_gemm`, `iggt_small_attention`, `iggt_layernorm`, with the AdaLN modulate in torch arithmetic.
+device-wide barrier separates the ~27 phases of an iteration).  Scenes of more than 16 views, devices with fewer than
+128 SMs (an H100 PCIe, a MIG slice) and IGGT_CAMERA_FUSED=0 run layer by layer: `iggt_skinny_gemm`,
+`iggt_small_attention`, `iggt_layernorm`, with the AdaLN modulate in torch arithmetic.
 """
 import ctypes
 import os
@@ -20,6 +21,21 @@ FUSED = os.environ.get("IGGT_CAMERA_FUSED", "1") != "0"
 
 DIM = 2048
 HEADS = 16
+FUSED_MIN_SMS = 128            # the one-launch kernel's grid holds every phase in <= 4 tiles per CTA only from 128 SMs
+
+_sm_counts = {}
+
+
+def _sm_count(device) -> int:
+    """Multiprocessor count of `device` (iggt_device_info), read once per device."""
+    idx = torch.device(device).index
+    idx = torch.cuda.current_device() if idx is None else idx
+    if idx not in _sm_counts:
+        n = ctypes.c_int(0)
+        with torch.cuda.device(idx):
+            _lib.check(_lib.load().iggt_device_info(None, ctypes.byref(n)), "iggt_device_info")
+        _sm_counts[idx] = n.value
+    return _sm_counts[idx]
 
 
 def _f32(p, device):
@@ -119,7 +135,7 @@ class CameraHead(Node):
         dt = compute_dtype or (torch.get_autocast_dtype("cuda") if torch.is_autocast_enabled("cuda") else torch.float16)
         pk = self._packed(dt, dev)
         M = B * S
-        if FUSED and S <= 16 and camera_tokens.is_cuda:
+        if FUSED and S <= 16 and camera_tokens.is_cuda and _sm_count(dev) >= FUSED_MIN_SMS:
             rows = camera_tokens.reshape(M, C)                    # a strided view of tokens[:, :, 0]: no copy
             if rows.dtype != torch.float32 or rows.stride(1) != 1:
                 rows = rows.float().contiguous()

@@ -176,7 +176,8 @@ int iggt_small_attention(const float* qkv, float* out, int B, int N, int H, int 
  * All weight matrices are 16-bit row-major [N, K] (torch Linear layout); vectors fp32.  tokens: fp32 camera-token rows,
  * row (b*S + s) at tokens + (b*S + s) * ld_tokens (ld_tokens = T*2048 reads layer 23's tokens[:, :, 0] in place).
  * out: fp32 [iters][B*S][9].  workspace: iggt_camera_head_workspace(B*S) bytes, 16-byte aligned.
- * Returns -7 when B*S > 16 (use the per-layer launchers). */
+ * Returns -7 when B*S > 16, or on a device with fewer than 128 SMs (a CTA would own more than the 4 tiles of a phase
+ * its consumers hold): use the per-layer launchers. */
 typedef struct {
   const float *n1w, *n1b; const void* qkv_w; const float* qkv_b; const void* proj_w; const float* proj_b; const float* ls1;
   const float *n2w, *n2b; const void* fc1_w; const float* fc1_b; const void* fc2_w; const float* fc2_b; const float* ls2;

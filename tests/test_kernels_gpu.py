@@ -344,26 +344,6 @@ def test_stride2_conv_as_im2col_gemm(ops, dtype):
 
 
 @pytest.mark.parametrize("dtype", DTYPES)
-@pytest.mark.parametrize("oc,mode", [(2, 0), (4, 1), (8, 2)])
-def test_dpt_tail(ops, dtype, oc, mode):
-    g = torch.Generator(device="cuda").manual_seed(29)
-    NB, H, W = 2, 9, 11
-    x = torch.randn(NB, H, W, 32, device="cuda", generator=g).to(dtype)
-    w = torch.randn(oc, 32, device="cuda", generator=g) / 6
-    b = torch.randn(oc, device="cuda", generator=g) * 0.1
-    main, conf = ops.dpt_tail(x, w, b, mode)
-    torch.cuda.synchronize()
-    o = x.float() @ w.t() + b
-    if mode == 2:
-        assert conf is None and _relmax(main, o.permute(0, 3, 1, 2)) < 1e-5
-    else:
-        xyz = o[..., :-1]
-        ref = torch.exp(xyz) if mode == 0 else torch.sign(xyz) * torch.expm1(xyz.abs())
-        assert ((main - ref).abs() / ref.abs().clamp_min(1e-3)).max().item() < 1e-4   # fp32 exp/expm1
-        assert ((conf - (1 + o[..., -1].exp())).abs() / (1 + o[..., -1].exp())).max().item() < 1e-5
-
-
-@pytest.mark.parametrize("dtype", DTYPES)
 @pytest.mark.parametrize("M,N,K,act", [(8, 2048, 2048, 0), (3, 9, 1024, 0), (20, 6144, 16, 4), (32, 1024, 8192, 1)])
 def test_skinny_gemm(ops, dtype, M, N, K, act):
     g = torch.Generator(device="cuda").manual_seed(31)
@@ -462,23 +442,3 @@ def test_window_attention(ops, dtype):
     o = (torch.softmax(q @ k.transpose(-2, -1) * (c // heads) ** -0.5, -1) @ v).transpose(1, 2).reshape(-1, 64, c)
     ref = ref_model.window_reverse(o.view(-1, 8, 8, c), 8, h, w)
     assert _relmax(out, ref) < 2 * _tol(dtype)
-
-
-@pytest.mark.parametrize("dtype", DTYPES)
-def test_channel_attention_pieces(ops, dtype):
-    g = torch.Generator(device="cuda").manual_seed(59)
-    NB, h, w, C, R = 3, 24, 16, 128, 4
-    y0 = torch.randn(NB, h, w, C, device="cuda", generator=g).to(dtype)
-    cx = torch.randn(NB, h, w, C, device="cuda", generator=g).to(dtype)
-    w1 = torch.randn(R, C, device="cuda", generator=g) / 8
-    b1 = torch.randn(R, device="cuda", generator=g)
-    w2 = torch.randn(C, R, device="cuda", generator=g)
-    b2 = torch.randn(C, device="cuda", generator=g)
-    mean = ops.channel_mean(cx)
-    out = ops.se_scale_add(y0, cx, mean, w1, b1, w2, b2, 0.01)
-    torch.cuda.synchronize()
-    m = cx.float().mean((1, 2))
-    assert _relmax(mean, m) < 1e-4
-    s = torch.sigmoid(F.relu(m @ w1.t() + b1) @ w2.t() + b2)
-    ref = y0.float() + 0.01 * cx.float() * s[:, None, None, :]
-    assert _relmax(out, ref) < _tol(dtype)
