@@ -91,6 +91,19 @@ SIGNATURES = {
                       c_void_p],
     "iggt_pca_stretch": [c_void_p, c_int64, c_int64, c_void_p, c_void_p, c_void_p],
     "iggt_sym_eig": [c_void_p, c_int, c_void_p, c_void_p],
+    "iggt_select": [c_void_p, c_int64, c_int64, c_int64, c_void_p, c_int64, c_int, ctypes.POINTER(c_float), c_int,
+                    c_void_p, c_void_p, c_void_p, c_void_p],
+    "iggt_quantile_rule": [c_void_p, c_int64, c_int, c_float, ctypes.POINTER(c_float)],
+    "iggt_resize_nearest": [c_void_p, c_int, c_int, c_int, c_void_p, c_int, c_int, c_void_p],
+    "iggt_zoom_nearest_index": [c_int, c_int, c_void_p],
+    "iggt_depth_valid_mask": [c_void_p, c_void_p, c_int64, c_int64, c_int, c_void_p, c_void_p],
+    "iggt_depth_metrics_workspace": [c_int64, ctypes.POINTER(c_int64)],
+    "iggt_depth_metrics": [c_void_p, c_void_p, c_void_p, c_int64, c_int64, c_int, c_void_p, c_int, c_float, c_float,
+                           c_int, c_void_p, c_void_p, c_void_p, c_void_p],
+    "iggt_pose_errors": [c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_void_p],
+    "iggt_pose_errors_host": [c_void_p, c_void_p, c_int, c_void_p, c_void_p],
+    "iggt_depth_zero_outside": [c_void_p, c_int64, c_int64, c_void_p, c_int, c_int, c_float, c_void_p],
+    "iggt_depth_to_cam": [c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p],
     "iggt_avgpool2_nhwc": [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p],
     "iggt_sample_bilinear_nhwc": [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p],
     "iggt_corr_sample": [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int,

@@ -25,6 +25,7 @@
 #include <algorithm>
 
 #include "../../include/iggt_b200.h"
+#include "fpops.cuh"
 #include "launch.cuh"
 
 namespace iggt {
@@ -34,45 +35,6 @@ constexpr int PCA_TILE = 256;         // points per tile = threads per CTA of th
 constexpr int PCA_MAX_CTAS = 1024;    // partial-sum slots in the basis workspace
 constexpr int PCA_JACOBI_SWEEPS = 64;
 constexpr int pca_nv(int c) { return c + c * (c + 1) / 2; }   // sums of d, then of d d^T (upper triangle, row-major)
-
-// ---- fp64 with one rounding per operation on the host and on the device.  nvcc would contract a * b + c into an
-// fma in device code; the intrinsics keep the device build operation for operation equal to the host build (whose
-// x86-64 baseline target has no fma to contract into), so both give bit-identical eigenvectors.
-__host__ __device__ __forceinline__ double dmul(double a, double b) {
-#ifdef __CUDA_ARCH__
-  return __dmul_rn(a, b);
-#else
-  return a * b;
-#endif
-}
-__host__ __device__ __forceinline__ double dadd(double a, double b) {
-#ifdef __CUDA_ARCH__
-  return __dadd_rn(a, b);
-#else
-  return a + b;
-#endif
-}
-__host__ __device__ __forceinline__ double dsub(double a, double b) {
-#ifdef __CUDA_ARCH__
-  return __dsub_rn(a, b);
-#else
-  return a - b;
-#endif
-}
-__host__ __device__ __forceinline__ double ddiv(double a, double b) {
-#ifdef __CUDA_ARCH__
-  return __ddiv_rn(a, b);
-#else
-  return a / b;
-#endif
-}
-__host__ __device__ __forceinline__ double dsqrt(double a) {
-#ifdef __CUDA_ARCH__
-  return __dsqrt_rn(a);
-#else
-  return sqrt(a);
-#endif
-}
 
 __host__ __device__ __forceinline__ void jacobi_sync() {
 #ifdef __CUDA_ARCH__
@@ -372,9 +334,66 @@ __device__ __forceinline__ float key_float(uint32_t k) {
   return __uint_as_float((k & 0x80000000u) ? (k & 0x7fffffffu) : ~k);
 }
 
-struct QsTargets {                    // one selection: QS_SLOTS target ranks, two quantiles
-  int64_t rank[QS_SLOTS];             // targets 2i, 2i + 1 = floor and ceil rank of quantile i
-  float weight[2];
+// ---- rank and interpolation rules of the selection (IGGT_QRULE_* in the header), shared by the device selection and
+// the host entry point iggt_quantile_rule, with one rounding per operation on both sides (fpops.cuh; fmaf below is an
+// explicit, correctly rounded fma on both).
+struct QsRank {
+  int64_t lo, hi;                     // order statistics (0-based ranks among the `count` selected values)
+  float w;                            // interpolation weight
+};
+
+// Ranks of quantile q among `count` > 0 values.
+//   TORCH: torch.quantile, q in [0, 1]: r = q * float32(n - 1) in fp32, floor / ceil, w = r - floor (clamped to n - 1).
+//   NUMPY, NUMPY_NAN: np.percentile / np.nanpercentile, method "linear", q in percent, as numpy 2.3 runs them for
+//     float32 data: q / float32(100) in fp32 (percentile divides by a.dtype.type(100)); virtual index
+//     v = float32(n - 1) * q in fp32 (n - 1 is a weak Python int); v >= n - 1 takes the last value twice with
+//     w = v - (-1) (numpy's index -1); otherwise lo = floor(v), hi = float32(lo + 1) (both still fp32, so above 2^24
+//     hi can round to lo or to lo + 2), w = v - lo.  hi is clamped to n - 1 where numpy would index past the end.
+//   MEDIAN: np.median: the middle value, or the two middle values of an even count.
+__host__ __device__ inline QsRank qs_rank(int rule, int64_t count, float q) {
+  QsRank k;
+  const int64_t last = count - 1;
+  if (rule == IGGT_QRULE_TORCH) {
+    const float r = fmul(q, static_cast<float>(last));
+    const int64_t lo = static_cast<int64_t>(r), hi = static_cast<int64_t>(ceilf(r));
+    k.lo = lo < last ? lo : last;                        // float32(n - 1) may round above n - 1 for n > 2^24
+    k.hi = hi < last ? hi : last;
+    k.w = fsub(r, static_cast<float>(lo));
+  } else if (rule == IGGT_QRULE_MEDIAN) {
+    k.lo = (count - 1) / 2;
+    k.hi = count / 2;
+    k.w = 0.f;
+  } else {
+    const float fl = static_cast<float>(last);
+    const float v = fmul(fl, fdiv(q, 100.f));
+    if (v >= fl) {
+      k.lo = k.hi = last;
+      k.w = fadd(v, 1.f);
+    } else {
+      const float lo = floorf(v), hi = fadd(lo, 1.f);
+      k.lo = static_cast<int64_t>(lo);
+      k.hi = static_cast<int64_t>(hi) < last ? static_cast<int64_t>(hi) : last;
+      k.w = fsub(v, lo);
+    }
+  }
+  return k;
+}
+
+// The quantile from the order statistics a (rank lo) and b (rank hi).
+//   TORCH: ATen's lerp (Lerp.h): the small-weight and large-weight branches, each a single fma as nvcc contracts them.
+//   NUMPY*: numpy's _lerp, no fma: d = b - a; a + d * w, or b - d * (1 - w) where w >= 0.5.
+//   MEDIAN: np.mean of the middle value(s) in fp32: a, or (a + b) / 2.
+__host__ __device__ inline float qs_interp(int rule, int64_t lo, int64_t hi, float a, float b, float w) {
+  if (rule == IGGT_QRULE_TORCH)
+    return fabsf(w) < 0.5f ? fmaf(w, fsub(b, a), a) : fmaf(-fsub(b, a), fsub(1.f, w), b);
+  if (rule == IGGT_QRULE_MEDIAN) return lo == hi ? a : fdiv(fadd(a, b), 2.f);
+  const float d = fsub(b, a);
+  return w >= 0.5f ? fsub(b, fmul(d, fsub(1.f, w))) : fadd(a, fmul(d, w));
+}
+
+struct QsTargets {                    // one selection: two quantiles (floor and ceil rank of each = QS_SLOTS targets)
+  float q[2];
+  int rule;
   int nout;                           // quantiles written (1 or 2)
 };
 struct QsRow {                        // per-row selection state between passes
@@ -382,7 +401,9 @@ struct QsRow {                        // per-row selection state between passes
   int nslots;
   int slot[QS_SLOTS];                 // prefix slot of each target
   int64_t rank[QS_SLOTS];             // rank of each target within its prefix
-  int has_nan;
+  int64_t order[QS_SLOTS];            // rank of each target among the selected values
+  float weight[2];
+  int nan_out;                        // the row's result is NaN (a NaN the rule propagates, or nothing selected)
 };
 
 // Histogram of one digit of every key (pass 0: bits 31..21) or of the keys under a slot's prefix (pass 1: bits
@@ -390,8 +411,8 @@ struct QsRow {                        // per-row selection state between passes
 // loads.  Counts go to shared memory (32 KB: pass 0 one copy per warp, later passes one per slot), then to hist.
 template <int PASS>
 __global__ void __launch_bounds__(QS_THREADS)
-qs_hist_kernel(const float* __restrict__ y, int64_t n, int64_t ld, const QsRow* __restrict__ state,
-               uint32_t* __restrict__ hist) {
+qs_hist_kernel(const float* __restrict__ y, int64_t n, int64_t ld, const uint8_t* __restrict__ mask, int64_t ldm,
+               const QsRow* __restrict__ state, uint32_t* __restrict__ hist) {
   __shared__ uint32_t h[QS_SLOTS][QS_BINS];
   const int row = blockIdx.y, t = threadIdx.x, warp = t >> 5;
   for (int i = t; i < QS_SLOTS * QS_BINS; i += QS_THREADS) (&h[0][0])[i] = 0;
@@ -403,7 +424,9 @@ qs_hist_kernel(const float* __restrict__ y, int64_t n, int64_t ld, const QsRow* 
     for (int s = 0; s < QS_SLOTS; ++s) pre[s] = state[row].prefix[s];
   }
   __syncthreads();
-  auto count = [&](float f) {
+  const uint8_t* m = mask ? mask + static_cast<int64_t>(row) * ldm : nullptr;
+  auto count = [&](float f, int64_t i) {
+    if (m && !m[i]) return;
     const uint32_t k = float_key(f);
     if (PASS == 0) {
       atomicAdd(&h[warp][k >> 21], 1u);
@@ -419,15 +442,16 @@ qs_hist_kernel(const float* __restrict__ y, int64_t n, int64_t ld, const QsRow* 
   const int64_t g = static_cast<int64_t>(blockIdx.x) * QS_THREADS + t;
   const int64_t stride = static_cast<int64_t>(gridDim.x) * QS_THREADS;
   const int64_t head = min(n, static_cast<int64_t>(((16 - (reinterpret_cast<uintptr_t>(r) & 15)) & 15) / 4));
-  if (g < head) count(r[g]);
+  if (g < head) count(r[g], g);
   const int64_t nv = (n - head) / 4;
   const float4* r4 = reinterpret_cast<const float4*>(r + head);
 #pragma unroll 4
   for (int64_t i = g; i < nv; i += stride) {
     const float4 v = __ldg(r4 + i);
-    count(v.x); count(v.y); count(v.z); count(v.w);
+    const int64_t e = head + 4 * i;
+    count(v.x, e); count(v.y, e + 1); count(v.z, e + 2); count(v.w, e + 3);
   }
-  for (int64_t i = head + 4 * nv + g; i < n; i += stride) count(r[i]);
+  for (int64_t i = head + 4 * nv + g; i < n; i += stride) count(r[i], i);
   __syncthreads();
   uint32_t* gh = hist + static_cast<int64_t>(row) * QS_SLOTS * QS_BINS;
   if (PASS == 0) {
@@ -444,23 +468,38 @@ qs_hist_kernel(const float* __restrict__ y, int64_t n, int64_t ld, const QsRow* 
 }
 
 // One warp per row: the bin of every target rank in its slot's histogram; the refined prefixes become the next
-// pass's slots.  After pass 2 the keys are complete: lerp of the floor / ceil order statistics, as ATen's lerp
-// (Lerp.h) computes it - the small-weight and large-weight branches, each a single fma as nvcc contracts them.
+// pass's slots.  Pass 0 first counts the row's selected values (all bins; NaN keys sit in the last bin alone) and
+// derives the target ranks from that count by qs_rank.  After pass 2 the keys are complete: qs_interp of the order
+// statistics.
 template <int PASS>
 __global__ void __launch_bounds__(32)
 qs_select_kernel(const uint32_t* __restrict__ hist, QsRow* __restrict__ state, QsTargets tg, float* __restrict__ out,
-                 int64_t ldo) {
+                 int64_t ldo, int64_t* __restrict__ count_out) {
   constexpr int BITS = PASS == 2 ? 10 : 11;
   constexpr int BINS = 1 << BITS;
   constexpr int PER_LANE = BINS / 32;
   const int row = blockIdx.x, lane = threadIdx.x;
   QsRow st;
   if (PASS == 0) {
+    const uint32_t* h0 = hist + static_cast<int64_t>(row) * QS_SLOTS * QS_BINS;
+    int64_t total = 0;
+    for (int b = lane; b < QS_BINS; b += 32) total += h0[b];
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) total += __shfl_xor_sync(0xffffffffu, total, o);
+    const int64_t nans = h0[QS_BINS - 1];                // NaN keys only
+    const int64_t count = tg.rule == IGGT_QRULE_NUMPY_NAN ? total - nans : total;
     st.nslots = 1;
     st.prefix[0] = 0;
+    st.nan_out = count == 0 || (tg.rule != IGGT_QRULE_NUMPY_NAN && nans != 0);
+    for (int q = 0; q < 2; ++q) {
+      const QsRank k = count > 0 ? qs_rank(tg.rule, count, tg.q[q]) : QsRank{0, 0, 0.f};
+      st.order[2 * q] = k.lo;
+      st.order[2 * q + 1] = k.hi;
+      st.weight[q] = k.w;
+    }
 #pragma unroll
-    for (int i = 0; i < QS_SLOTS; ++i) { st.slot[i] = 0; st.rank[i] = tg.rank[i]; }
-    st.has_nan = hist[static_cast<int64_t>(row) * QS_SLOTS * QS_BINS + QS_BINS - 1] != 0;   // NaN keys only
+    for (int i = 0; i < QS_SLOTS; ++i) { st.slot[i] = 0; st.rank[i] = st.order[i]; }
+    if (count_out && lane == 0) count_out[row] = count;
   } else {
     st = state[row];
   }
@@ -498,8 +537,7 @@ qs_select_kernel(const uint32_t* __restrict__ hist, QsRow* __restrict__ state, Q
   }
   if (lane != 0) return;
   if (PASS < 2) {
-    QsRow nx;
-    nx.has_nan = st.has_nan;
+    QsRow nx = st;
     nx.nslots = 0;
     for (int i = 0; i < QS_SLOTS; ++i) {
       int s = 0;
@@ -511,14 +549,9 @@ qs_select_kernel(const uint32_t* __restrict__ hist, QsRow* __restrict__ state, Q
     state[row] = nx;
   } else {
     for (int q = 0; q < tg.nout; ++q) {
-      float r;
-      if (st.has_nan) {
-        r = __uint_as_float(0x7fc00000u);
-      } else {
-        const float self = key_float(key[2 * q]), end = key_float(key[2 * q + 1]), w = tg.weight[q];
-        r = fabsf(w) < 0.5f ? __fmaf_rn(w, __fsub_rn(end, self), self)
-                            : __fmaf_rn(-__fsub_rn(end, self), __fsub_rn(1.f, w), end);
-      }
+      const float r = st.nan_out ? __uint_as_float(0x7fc00000u)
+                                 : qs_interp(tg.rule, st.order[2 * q], st.order[2 * q + 1], key_float(key[2 * q]),
+                                             key_float(key[2 * q + 1]), st.weight[q]);
       out[static_cast<int64_t>(row) * ldo + q] = r;
     }
   }
@@ -610,13 +643,9 @@ extern "C" int iggt_quantile_workspace(int64_t rows, int64_t* bytes) {
   return 0;
 }
 
-extern "C" int iggt_quantile(const float* y, int64_t rows, int64_t n, int64_t ld, const float* q, int nq,
-                             void* workspace, float* out, iggt_stream_t stream) {
-  if (!y || !q || !workspace || !out || rows <= 0 || rows > 65535 || n <= 0 || n >= (1LL << 32) || ld < n || nq <= 0)
-    return -1;
-  for (int i = 0; i < nq; ++i)
-    if (!(q[i] >= 0.f && q[i] <= 1.f)) return -1;
-  cudaStream_t st = (cudaStream_t)stream;
+// The radix selection behind iggt_quantile and iggt_select: every row, one pair of quantiles per three passes.
+static int qs_run(const float* y, int64_t rows, int64_t n, int64_t ld, const uint8_t* mask, int64_t ldm, int rule,
+                  const float* q, int nq, void* workspace, float* out, int64_t* count, cudaStream_t st) {
   uint32_t* hist = static_cast<uint32_t*>(workspace);
   const int64_t hb = qs_hist_bytes(rows);
   QsRow* state = reinterpret_cast<QsRow*>(static_cast<char*>(workspace) + 3 * hb);
@@ -626,27 +655,64 @@ extern "C" int iggt_quantile(const float* y, int64_t rows, int64_t n, int64_t ld
   const dim3 hgrid(static_cast<unsigned>(std::min<int64_t>(gx, std::max<int64_t>(chunks, 1))), static_cast<unsigned>(rows));
   const int R = static_cast<int>(rows);
   for (int q0 = 0; q0 < nq; q0 += 2) {
-    // torch.quantile: rank = float32(q) * float32(n - 1) in fp32; floor / ceil order statistics; weight = rank - floor
     QsTargets tg;
+    tg.rule = rule;
     tg.nout = nq - q0 < 2 ? nq - q0 : 2;
-    for (int i = 0; i < 2; ++i) {
-      const float r = q[q0 + (i < tg.nout ? i : 0)] * static_cast<float>(n - 1);
-      const int64_t lo = static_cast<int64_t>(r), hi = static_cast<int64_t>(ceilf(r));
-      tg.rank[2 * i] = lo < n - 1 ? lo : n - 1;          // float32(n - 1) may round above n - 1 for n > 2^24
-      tg.rank[2 * i + 1] = hi < n - 1 ? hi : n - 1;
-      tg.weight[i] = r - static_cast<float>(lo);
-    }
+    for (int i = 0; i < 2; ++i) tg.q[i] = q[q0 + (i < tg.nout ? i : 0)];
     cudaError_t e = cudaMemsetAsync(hist, 0, 3 * hb, st);
     if (e != cudaSuccess) return (int)e;
-    qs_hist_kernel<0><<<hgrid, QS_THREADS, 0, st>>>(y, n, ld, state, hist);
-    qs_select_kernel<0><<<R, 32, 0, st>>>(hist, state, tg, out + q0, nq);
-    qs_hist_kernel<1><<<hgrid, QS_THREADS, 0, st>>>(y, n, ld, state, hist + hb / 4);
-    qs_select_kernel<1><<<R, 32, 0, st>>>(hist + hb / 4, state, tg, out + q0, nq);
-    qs_hist_kernel<2><<<hgrid, QS_THREADS, 0, st>>>(y, n, ld, state, hist + hb / 2);
-    qs_select_kernel<2><<<R, 32, 0, st>>>(hist + hb / 2, state, tg, out + q0, nq);
+    qs_hist_kernel<0><<<hgrid, QS_THREADS, 0, st>>>(y, n, ld, mask, ldm, state, hist);
+    qs_select_kernel<0><<<R, 32, 0, st>>>(hist, state, tg, out + q0, nq, q0 == 0 ? count : nullptr);
+    qs_hist_kernel<1><<<hgrid, QS_THREADS, 0, st>>>(y, n, ld, mask, ldm, state, hist + hb / 4);
+    qs_select_kernel<1><<<R, 32, 0, st>>>(hist + hb / 4, state, tg, out + q0, nq, nullptr);
+    qs_hist_kernel<2><<<hgrid, QS_THREADS, 0, st>>>(y, n, ld, mask, ldm, state, hist + hb / 2);
+    qs_select_kernel<2><<<R, 32, 0, st>>>(hist + hb / 2, state, tg, out + q0, nq, nullptr);
     e = cudaGetLastError();
     if (e != cudaSuccess) return (int)e;
   }
+  return 0;
+}
+
+extern "C" int iggt_quantile(const float* y, int64_t rows, int64_t n, int64_t ld, const float* q, int nq,
+                             void* workspace, float* out, iggt_stream_t stream) {
+  if (!y || !q || !workspace || !out || rows <= 0 || rows > 65535 || n <= 0 || n >= (1LL << 32) || ld < n || nq <= 0)
+    return -1;
+  for (int i = 0; i < nq; ++i)
+    if (!(q[i] >= 0.f && q[i] <= 1.f)) return -1;
+  return qs_run(y, rows, n, ld, nullptr, 0, IGGT_QRULE_TORCH, q, nq, workspace, out, nullptr, (cudaStream_t)stream);
+}
+
+extern "C" int iggt_select(const float* y, int64_t rows, int64_t n, int64_t ld, const uint8_t* mask, int64_t ldm,
+                           int rule, const float* q, int nq, void* workspace, float* out, int64_t* count,
+                           iggt_stream_t stream) {
+  if (!y || !workspace || !out || rows <= 0 || rows > 65535 || n <= 0 || n >= (1LL << 32) || ld < n ||
+      (mask && ldm < n) || rule < IGGT_QRULE_TORCH || rule > IGGT_QRULE_MEDIAN)
+    return -1;
+  const float median_q = 0.f;
+  if (rule == IGGT_QRULE_MEDIAN) {
+    if (nq != 1) return -1;
+    q = &median_q;
+  } else {
+    if (!q || nq <= 0) return -1;
+    const float qmax = rule == IGGT_QRULE_TORCH ? 1.f : 100.f;
+    for (int i = 0; i < nq; ++i)
+      if (!(q[i] >= 0.f && q[i] <= qmax)) return -1;
+  }
+  return qs_run(y, rows, n, ld, mask, ldm, rule, q, nq, workspace, out, count, (cudaStream_t)stream);
+}
+
+extern "C" int iggt_quantile_rule(const float* sorted, int64_t count, int rule, float q, float* out) {
+  if (!out || count < 0 || (count > 0 && !sorted) || rule < IGGT_QRULE_TORCH || rule > IGGT_QRULE_MEDIAN) return -1;
+  if (rule != IGGT_QRULE_MEDIAN && !(q >= 0.f && q <= (rule == IGGT_QRULE_TORCH ? 1.f : 100.f))) return -1;
+  int64_t nans = 0;                                      // NaNs sort last, as np.sort puts them
+  while (nans < count && isnan(sorted[count - 1 - nans])) ++nans;
+  const int64_t n = rule == IGGT_QRULE_NUMPY_NAN ? count - nans : count;
+  if (n == 0 || (rule != IGGT_QRULE_NUMPY_NAN && nans != 0)) {
+    *out = NAN;
+    return 0;
+  }
+  const QsRank k = qs_rank(rule, n, q);
+  *out = qs_interp(rule, k.lo, k.hi, sorted[k.lo], sorted[k.hi], k.w);
   return 0;
 }
 

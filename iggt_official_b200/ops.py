@@ -680,6 +680,148 @@ def sym_eig(a):
 
 
 # ---------------------------------------------------------------------------------------------------
+# Scene evaluation (csrc/evaluate.cu; the selection in csrc/pca.cu)
+QRULE_TORCH, QRULE_NUMPY, QRULE_NUMPY_NAN, QRULE_MEDIAN = 0, 1, 2, 3
+ALIGN_NONE, ALIGN_MEDIAN, ALIGN_LSQ = 0, 1, 2
+EVAL_RECORD = 16
+
+
+def select(y, rule, q=(), mask=None, return_count=False):
+    """y [rows,n] fp32 (unit column stride), optional mask [rows,n] uint8/bool -> [rows, len(q)] fp32: the quantiles
+    of each row's masked-in values under `rule` (QRULE_*; percentages for the numpy rules; QRULE_MEDIAN takes no q),
+    bit for bit numpy's for float32 data.  With return_count, also the selected count per row (int64)."""
+    import ctypes
+    assert y.is_cuda and y.dtype == torch.float32 and y.dim() == 2 and y.stride(1) == 1
+    rows, n = y.shape
+    q = [0.0] if rule == QRULE_MEDIAN else [float(v) for v in q]
+    assert 0 < rows <= 65535 and 0 < n < 2 ** 32 and len(q) > 0
+    if mask is not None:
+        assert mask.is_cuda and mask.shape == y.shape and mask.dtype in (torch.uint8, torch.bool)
+        mask = mask.view(torch.uint8) if mask.dtype == torch.bool else mask
+        assert mask.stride(1) == 1
+    ws = torch.empty(_workspace("iggt_quantile_workspace", rows), dtype=torch.uint8, device=y.device)
+    out = torch.empty((rows, len(q)), dtype=torch.float32, device=y.device)
+    count = torch.empty(rows, dtype=torch.int64, device=y.device) if return_count else None
+    qa = (ctypes.c_float * len(q))(*q)
+    _call(y, "iggt_select", 0, 5.0 * rows * n * 3 * ((len(q) + 1) // 2), y.data_ptr(), rows, n, y.stride(0),
+          _ptr(mask), 0 if mask is None else mask.stride(0), rule, qa, len(q), ws.data_ptr(), out.data_ptr(),
+          _ptr(count), _STREAM)
+    return (out, count) if return_count else out
+
+
+def quantile_rule(sorted_values, rule, q=0.0):
+    """Host (no GPU): the quantile of an ascending float32 array (NaNs last) under `rule`, by the rank and
+    interpolation code the device selection runs."""
+    import ctypes
+    import numpy as np
+    a = np.ascontiguousarray(sorted_values, dtype=np.float32)
+    out = ctypes.c_float()
+    _lib.check(_lib.load().iggt_quantile_rule(a.ctypes.data, a.size, rule, float(q), ctypes.byref(out)),
+               "iggt_quantile_rule")
+    return np.float32(out.value)
+
+
+def resize_nearest(src, Ho, Wo):
+    """src [S,Hi,Wi] fp32 -> [S,Ho,Wo]: skimage.transform.resize(order=0, anti_aliasing=False)'s nearest samples, by
+    scipy.ndimage.zoom(order=0, grid_mode=True)'s index map."""
+    assert src.is_cuda and src.dtype == torch.float32 and src.dim() == 3
+    src = src.contiguous()
+    S, Hi, Wi = src.shape
+    dst = torch.empty((S, Ho, Wo), dtype=torch.float32, device=src.device)
+    _call(src, "iggt_resize_nearest", 0, 8.0 * S * Ho * Wo, src.data_ptr(), S, Hi, Wi, dst.data_ptr(), Ho, Wo, _STREAM)
+    return dst
+
+
+def zoom_nearest_index(n_in, n_out):
+    """Host (no GPU): int32 [n_out], the source index of every output index of resize_nearest along one axis."""
+    import numpy as np
+    idx = np.empty(n_out, np.int32)
+    _lib.check(_lib.load().iggt_zoom_nearest_index(int(n_in), int(n_out), idx.ctypes.data), "iggt_zoom_nearest_index")
+    return idx
+
+
+def depth_valid_mask(gt, pred, sparse):
+    """gt, pred [S,n] fp32 -> uint8 [S,n] = gt > 0 & (pred != 0 if sparse)."""
+    assert gt.is_cuda and gt.dtype == pred.dtype == torch.float32 and gt.shape == pred.shape and gt.dim() == 2
+    gt, pred = gt.contiguous(), pred.contiguous()
+    mask = torch.empty(gt.shape, dtype=torch.uint8, device=gt.device)
+    _call(gt, "iggt_depth_valid_mask", 0, 9.0 * gt.numel(), gt.data_ptr(), pred.data_ptr(), gt.shape[0], gt.shape[1],
+          int(bool(sparse)), mask.data_ptr(), _STREAM)
+    return mask
+
+
+def depth_metrics(gt, pred, mask, alignment, medians=None, clip=None, sparse=False, want_aligned=False):
+    """gt, pred [S,n] fp32, mask [S,n] uint8 -> (records [S, EVAL_RECORD] fp64 on the device, aligned [S,n] or None).
+    medians [2,S] fp32 (GT row, prediction row) for ALIGN_MEDIAN; clip = (lo, hi) or None."""
+    assert gt.is_cuda and gt.dtype == pred.dtype == torch.float32 and gt.shape == pred.shape and gt.dim() == 2
+    assert mask.shape == gt.shape and mask.dtype == torch.uint8
+    gt, pred, mask = gt.contiguous(), pred.contiguous(), mask.contiguous()
+    S, n = gt.shape
+    if alignment == ALIGN_MEDIAN:
+        assert medians is not None and medians.shape == (2, S) and medians.dtype == torch.float32
+        medians = medians.contiguous()
+    ws = torch.empty(_workspace("iggt_depth_metrics_workspace", S), dtype=torch.uint8, device=gt.device)
+    rec = torch.empty((S, EVAL_RECORD), dtype=torch.float64, device=gt.device)
+    aligned = torch.empty_like(gt) if want_aligned else None
+    lo, hi = (0.0, 0.0) if clip is None else (float(clip[0]), float(clip[1]))
+    passes = 2 if alignment == ALIGN_LSQ else 1
+    _call(gt, "iggt_depth_metrics", 20.0 * S * n, 9.0 * S * n * passes, gt.data_ptr(), pred.data_ptr(),
+          mask.data_ptr(), S, n, int(alignment), _ptr(medians), int(clip is not None), lo, hi, int(bool(sparse)),
+          ws.data_ptr(), rec.data_ptr(), _ptr(aligned), _STREAM)
+    return rec, aligned
+
+
+def pose_errors(gt, pred):
+    """gt, pred [N,3,4] fp64 CUDA -> (translation errors [N], rotation errors [N] in degrees), fp64."""
+    assert gt.is_cuda and gt.dtype == pred.dtype == torch.float64 and gt.shape == pred.shape and gt.shape[1:] == (3, 4)
+    gt, pred = gt.contiguous(), pred.contiguous()
+    N = gt.shape[0]
+    t = torch.empty(N, dtype=torch.float64, device=gt.device)
+    r = torch.empty(N, dtype=torch.float64, device=gt.device)
+    _call(gt, "iggt_pose_errors", 200.0 * N, 224.0 * N, gt.data_ptr(), pred.data_ptr(), N, t.data_ptr(), r.data_ptr(),
+          _STREAM)
+    return t, r
+
+
+def pose_errors_host(gt, pred):
+    """Host (no GPU): pose_errors on float64 ndarrays [N,3,4], the same code."""
+    import numpy as np
+    gt = np.ascontiguousarray(gt, dtype=np.float64)
+    pred = np.ascontiguousarray(pred, dtype=np.float64)
+    assert gt.shape == pred.shape and gt.shape[1:] == (3, 4)
+    N = gt.shape[0]
+    t, r = np.empty(N), np.empty(N)
+    _lib.check(_lib.load().iggt_pose_errors_host(gt.ctypes.data, pred.ctypes.data, N, t.ctypes.data, r.ctypes.data),
+               "iggt_pose_errors_host")
+    return t, r
+
+
+def depth_zero_outside(depth, thr=None, use_hi=True, use_lo=True, max_depth=-1.0):
+    """In place on depth [S,n] fp32 (contiguous): thr None -> zero values > max_depth; else zero values > thr[s,0]
+    (use_hi, thr > 0) and < thr[s,1] (use_lo, thr > 0), thr [S,2] fp32 on the device."""
+    assert depth.is_cuda and depth.dtype == torch.float32 and depth.dim() == 2 and depth.is_contiguous()
+    S, n = depth.shape
+    if thr is not None:
+        assert thr.shape == (S, 2) and thr.dtype == torch.float32
+        thr = thr.contiguous()
+    _call(depth, "iggt_depth_zero_outside", 0, 8.0 * S * n, depth.data_ptr(), S, n, _ptr(thr), int(bool(use_hi)),
+          int(bool(use_lo)), float(max_depth), _STREAM)
+    return depth
+
+
+def depth_to_cam(depth, intr):
+    """depth [S,H,W] fp32, intr [S,3,3] fp64 -> camera coordinates [S,H,W,3] fp32 (fp64 arithmetic, rounded once)."""
+    assert depth.is_cuda and depth.dtype == torch.float32 and depth.dim() == 3
+    depth = depth.contiguous()
+    S, H, W = depth.shape
+    intr = intr.to(device=depth.device, dtype=torch.float64).reshape(S, 3, 3).contiguous()
+    cam = torch.empty((S, H, W, 3), dtype=torch.float32, device=depth.device)
+    _call(depth, "iggt_depth_to_cam", 6.0 * S * H * W, 16.0 * S * H * W, depth.data_ptr(), intr.data_ptr(), S, H, W,
+          cam.data_ptr(), _STREAM)
+    return cam
+
+
+# ---------------------------------------------------------------------------------------------------
 # Track head (csrc/track.cu)
 def avgpool2_nhwc(x):
     """[NB,H,W,C] 16-bit -> [NB,H//2,W//2,C]."""

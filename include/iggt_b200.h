@@ -383,6 +383,30 @@ int iggt_quantile_workspace(int64_t rows, int64_t* bytes);
 int iggt_quantile(const float* y, int64_t rows, int64_t n, int64_t ld, const float* q, int nq, void* workspace,
                   float* out, iggt_stream_t stream);
 
+/* Rank / interpolation rules of iggt_select and iggt_quantile_rule. */
+#define IGGT_QRULE_TORCH 0      /* torch.quantile (q in [0, 1]); iggt_quantile's rule */
+#define IGGT_QRULE_NUMPY 1      /* np.percentile(a, q), method "linear", q in percent; a NaN gives NaN */
+#define IGGT_QRULE_NUMPY_NAN 2  /* np.nanpercentile(a, q): NaNs are left out; nothing left gives NaN */
+#define IGGT_QRULE_MEDIAN 3     /* np.median(a): (a + b) / 2 in fp32 for an even count; a NaN gives NaN */
+
+/* The selection behind iggt_quantile, generalised (metrics.py:336 np.median, datasets/utils/misc.py:528-533
+ * np.nanpercentile).  For every row r of y [rows, n] (row pitch ld), the values y[r, i] with mask[r, i] != 0 (mask
+ * uint8 [rows, n], row pitch ldm; NULL = every value) are selected, and out [rows, nq] gets quantile q[i] of them under
+ * `rule` (q a HOST array; for IGGT_QRULE_MEDIAN, q is ignored and nq = 1).  The target ranks are derived on the device
+ * from each row's selected count, by the rank rule of iggt_quantile_rule; count [rows] int64 (may be NULL) receives
+ * that count (NaNs left out under IGGT_QRULE_NUMPY_NAN).  An empty row gives NaN.  Bit for bit numpy 2.3 for float32
+ * data, except that -0 orders before +0 (numpy treats them as equal and may return either).  Workspace:
+ * iggt_quantile_workspace(rows). */
+int iggt_select(const float* y, int64_t rows, int64_t n, int64_t ld, const uint8_t* mask, int64_t ldm, int rule,
+                const float* q, int nq, void* workspace, float* out, int64_t* count, iggt_stream_t stream);
+
+/* HOST function (no GPU): *out = quantile q of sorted[0 .. count) (ascending, NaNs last, as np.sort orders them)
+ * under `rule`, by the same rank and interpolation code the device selection runs.  Rank rules for float32 data, as
+ * numpy 2.3 runs them: q32 = float32(q) / float32(100); v = float32(n - 1) * q32 in fp32; v >= n - 1 takes the last
+ * value with weight v + 1; else lo = floor(v), hi = float32(lo + 1), w = v - lo; numpy's _lerp without fma:
+ * a + (b - a) * w, or b - (b - a) * (1 - w) where w >= 0.5. */
+int iggt_quantile_rule(const float* sorted, int64_t count, int rule, float q, float* out);
+
 /* out [n, 3] = clamp((y[j, i] - lo_j) / (hi_j - lo_j), 0, 1), or 0.5 where hi_j <= lo_j, for y [3, n] (row pitch ldy)
  * and qv [3, 2] = (lo_j, hi_j) (device pointer, e.g. iggt_quantile's output for q = 0.02, 0.98). */
 int iggt_pca_stretch(const float* y, int64_t n, int64_t ldy, const float* qv, float* out, iggt_stream_t stream);
@@ -392,6 +416,68 @@ int iggt_pca_stretch(const float* y, int64_t n, int64_t ldy, const float* qv, fl
  * evecs [C, C] row-major with eigenvector j in column j, its largest-magnitude component positive (the first one
  * when several tie).  -1: a non-finite entry. */
 int iggt_sym_eig(const double* a, int C, double* evals, double* evecs);
+
+/* ---- Scene evaluation (iggt/metrics.py:257-671 DepthEvaluator / PoseEvaluator / SceneEvaluator, run per frame in
+ * numpy by demo.py:145-163) and the ground-truth depth helpers (csrc/evaluate.cu).  Depth maps are fp32 [S, n]. */
+
+/* Nearest-neighbour resize src [S, Hi, Wi] -> dst [S, Ho, Wo] (metrics.py:294-297:
+ * skimage.transform.resize(order=0, anti_aliasing=False)).  skimage >= 0.19 runs that as
+ * scipy.ndimage.zoom(order=0, grid_mode=True); the source index of output row / column k is scipy's
+ * floor(((k + 0.5) * (n_in / n_out) - 0.5) + 0.5) in fp64, clamped to [0, n_in - 1] (iggt_zoom_nearest_index).  The
+ * mapping is pinned to scipy's zoom, not checked against skimage itself. */
+int iggt_resize_nearest(const float* src, int S, int Hi, int Wi, float* dst, int Ho, int Wo, iggt_stream_t stream);
+
+/* HOST function (no GPU): idx [n_out] int32 = the source index of every output index, as iggt_resize_nearest maps it. */
+int iggt_zoom_nearest_index(int n_in, int n_out, int32_t* idx);
+
+/* mask [S, n] uint8 = gt > 0 and (if sparse) pred != 0 (metrics.py:300-302). */
+int iggt_depth_valid_mask(const float* gt, const float* pred, int64_t S, int64_t n, int sparse, uint8_t* mask,
+                          iggt_stream_t stream);
+
+#define IGGT_ALIGN_NONE 0
+#define IGGT_ALIGN_MEDIAN 1
+#define IGGT_ALIGN_LSQ 2
+#define IGGT_EVAL_RECORD 16     /* doubles per frame of iggt_depth_metrics' records */
+
+/* Host query: *bytes = device workspace size of iggt_depth_metrics for S frames. */
+int iggt_depth_metrics_workspace(int64_t S, int64_t* bytes);
+
+/* Per-frame depth metrics (metrics.py:82-165 and :299-409) of gt [S, n] against pred [S, n] (already at the GT
+ * resolution) over mask [S, n] (iggt_depth_valid_mask).  Alignment: MEDIAN takes medians [2, S] (row 0 the GT
+ * medians, row 1 the prediction medians over the mask, e.g. from iggt_select) and ratio = gt_med / pred_med in fp32;
+ * LSQ first sums gt * pred and pred^2 (fp32 products) over the mask, scale = float32(sum_gp / sum_pp).  A ratio that
+ * is not finite (LSQ: or not > 0) leaves the prediction as it is.  Then, in fp32 and numpy's operation order: the
+ * prediction times the ratio; with clip != 0, clip to [clip_lo, clip_hi] (NaN stays NaN) times the sparse mask; and
+ * per evaluated pixel (mask, and pred != 0 if sparse) the terms of m_rel_ae, thresh_inliers(1.03), mae, rmse and the
+ * delta ratios.  Sums are fp64: per-CTA partials added in a fixed order, so repeated calls are bit-identical.
+ * records [S, IGGT_EVAL_RECORD] fp64: 0 valid pixels, 1 evaluated pixels, 2 sum of |p - g| / g (non-finite -> 0),
+ * 3 inliers, 4 sum |g - p|, 5 sum (g - p)^2, 6 finite max(g/p, p/g), 7..9 of them below 1.25, 1.25^2, 1.25^3,
+ * 10 the ratio (1 if not applied), 11 1 if it was applied, 12 / 13 the GT / prediction medians (LSQ: the two sums).
+ * aligned (may be NULL): [S, n] the aligned, clipped prediction. */
+int iggt_depth_metrics(const float* gt, const float* pred, const uint8_t* mask, int64_t S, int64_t n, int alignment,
+                       const float* medians, int clip, float clip_lo, float clip_hi, int sparse, void* workspace,
+                       double* records, float* aligned, iggt_stream_t stream);
+
+/* Pose errors of N frames (metrics.py:436-525) from gt, pred [N, 3, 4] fp64 (the rows of [R | t]): t_err[i] =
+ * |t_gt - t_pred|, r_err[i] = the angle of R_gt^T R_pred in degrees, as scipy 1.18's
+ * Rotation.from_matrix(M).magnitude() computes it: M is replaced by its orthogonal polar factor (scipy: U V^T of
+ * the SVD) unless M M^T is within isclose(atol=1e-12, rtol=1e-5) of I; the quaternion by the largest of the diagonal
+ * and the trace; 2 atan2(|xyz|, |w|).  det(M) <= 0 gives NaN (scipy raises; the reference returns NaN). */
+int iggt_pose_errors(const double* gt, const double* pred, int N, double* t_err, double* r_err, iggt_stream_t stream);
+
+/* HOST function (no GPU): iggt_pose_errors on host arrays, the same code. */
+int iggt_pose_errors_host(const double* gt, const double* pred, int N, double* t_err, double* r_err);
+
+/* In place on depth [S, n] (datasets/utils/misc.py:524-539, threshold_depth_map): with thr == NULL, zero every value
+ * > max_depth; else zero values > thr[s, 0] where use_hi and thr[s, 0] > 0, and values < thr[s, 1] where use_lo and
+ * thr[s, 1] > 0 (thr [S, 2] fp32 device, e.g. iggt_select's nanpercentiles). */
+int iggt_depth_zero_outside(float* depth, int64_t S, int64_t n, const float* thr, int use_hi, int use_lo,
+                            float max_depth, iggt_stream_t stream);
+
+/* Camera coordinates cam [S, H, W, 3] fp32 of depth [S, H, W] (geometry.py:238-268 depth_to_cam_coords_points):
+ * ((u - cu) d / fu, (v - cv) d / fv, d) in fp64, one rounding per operation, rounded to fp32 (the reference's numpy
+ * promotes the pixel grid and the intrinsics to float64).  intr [S, 3, 3] fp64. */
+int iggt_depth_to_cam(const float* depth, const double* intr, int S, int H, int W, float* cam, iggt_stream_t stream);
 
 #ifdef __cplusplus
 }
