@@ -104,6 +104,11 @@ SIGNATURES = {
     "iggt_pose_errors_host": [c_void_p, c_void_p, c_int, c_void_p, c_void_p],
     "iggt_depth_zero_outside": [c_void_p, c_int64, c_int64, c_void_p, c_int, c_int, c_float, c_void_p],
     "iggt_depth_to_cam": [c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p],
+    "iggt_pointcloud_workspace": [c_int64, ctypes.POINTER(c_int64)],
+    "iggt_pointcloud_select": [c_void_p, c_void_p, c_int64, c_void_p, c_void_p, c_int, c_int64, c_int64, c_int64,
+                               c_int64, c_int, c_void_p, c_void_p, c_int64, c_void_p, c_void_p, c_void_p],
+    "iggt_pointcloud_compact": [c_void_p, c_void_p, c_void_p, c_int64, c_void_p, c_void_p, c_void_p, c_void_p,
+                                c_void_p],
     "iggt_avgpool2_nhwc": [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p],
     "iggt_sample_bilinear_nhwc": [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p],
     "iggt_corr_sample": [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int,

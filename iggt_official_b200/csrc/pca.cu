@@ -686,7 +686,7 @@ extern "C" int iggt_select(const float* y, int64_t rows, int64_t n, int64_t ld, 
                            int rule, const float* q, int nq, void* workspace, float* out, int64_t* count,
                            iggt_stream_t stream) {
   if (!y || !workspace || !out || rows <= 0 || rows > 65535 || n <= 0 || n >= (1LL << 32) || ld < n ||
-      (mask && ldm < n) || rule < IGGT_QRULE_TORCH || rule > IGGT_QRULE_MEDIAN)
+      (mask && ldm != 0 && ldm < n) || rule < IGGT_QRULE_TORCH || rule > IGGT_QRULE_MEDIAN)   // ldm 0: one shared row
     return -1;
   const float median_q = 0.f;
   if (rule == IGGT_QRULE_MEDIAN) {

@@ -686,10 +686,12 @@ ALIGN_NONE, ALIGN_MEDIAN, ALIGN_LSQ = 0, 1, 2
 EVAL_RECORD = 16
 
 
-def select(y, rule, q=(), mask=None, return_count=False):
+def select(y, rule, q=(), mask=None, return_count=False, out=None):
     """y [rows,n] fp32 (unit column stride), optional mask [rows,n] uint8/bool -> [rows, len(q)] fp32: the quantiles
     of each row's masked-in values under `rule` (QRULE_*; percentages for the numpy rules; QRULE_MEDIAN takes no q),
-    bit for bit numpy's for float32 data.  With return_count, also the selected count per row (int64)."""
+    bit for bit numpy's for float32 data.  With return_count, also the selected count per row (int64).  A mask
+    expanded from one row (row stride 0) is shared by every row.  out: an optional contiguous [rows, len(q)] fp32
+    tensor to write the result into."""
     import ctypes
     assert y.is_cuda and y.dtype == torch.float32 and y.dim() == 2 and y.stride(1) == 1
     rows, n = y.shape
@@ -700,7 +702,9 @@ def select(y, rule, q=(), mask=None, return_count=False):
         mask = mask.view(torch.uint8) if mask.dtype == torch.bool else mask
         assert mask.stride(1) == 1
     ws = torch.empty(_workspace("iggt_quantile_workspace", rows), dtype=torch.uint8, device=y.device)
-    out = torch.empty((rows, len(q)), dtype=torch.float32, device=y.device)
+    if out is None:
+        out = torch.empty((rows, len(q)), dtype=torch.float32, device=y.device)
+    assert out.dtype == torch.float32 and out.shape == (rows, len(q)) and out.is_contiguous() and out.device == y.device
     count = torch.empty(rows, dtype=torch.int64, device=y.device) if return_count else None
     qa = (ctypes.c_float * len(q))(*q)
     _call(y, "iggt_select", 0, 5.0 * rows * n * 3 * ((len(q) + 1) // 2), y.data_ptr(), rows, n, y.stride(0),
@@ -819,6 +823,57 @@ def depth_to_cam(depth, intr):
     _call(depth, "iggt_depth_to_cam", 6.0 * S * H * W, 16.0 * S * H * W, depth.data_ptr(), intr.data_ptr(), S, H, W,
           cam.data_ptr(), _STREAM)
     return cam
+
+
+# ---------------------------------------------------------------------------------------------------
+# Point-cloud export (csrc/pointcloud.cu; the selection in csrc/pca.cu)
+PC_COLOR_F32, PC_COLOR_U8 = 0, 1
+PC_MASK_BLACK, PC_MASK_WHITE = 1, 2
+
+
+def pointcloud_select(points, conf, thr, color, bg_flags=0):
+    """points [n,3] fp32, conf [n] fp32, thr: a one-element fp32 device tensor or None (0.0), color: fp32 / uint8,
+    NCHW [S,3,H,W] or channels-last [n,3], all contiguous -> (mask [n] uint8, planes [3,n] fp32 (16-byte aligned
+    rows), rgba [n] int32 (r | g << 8 | b << 16 | 255 << 24), workspace holding the tile counts for
+    pointcloud_compact)."""
+    assert points.is_cuda and points.dtype == torch.float32 and points.dim() == 2 and points.shape[1] == 3
+    assert points.is_contiguous() and conf.is_contiguous() and color.is_contiguous()
+    n = points.shape[0]
+    assert conf.dtype == torch.float32 and conf.shape == (n,) and 0 < n < 2 ** 32
+    assert color.dtype in (torch.float32, torch.uint8)
+    if color.dim() == 4:
+        S, C, H, W = color.shape
+        assert C == 3 and S * H * W == n
+        geom = (H * W, 3 * H * W, H * W, 1)
+    else:
+        assert color.shape == (n, 3)
+        geom = (n, 0, 1, 3)
+    kind = PC_COLOR_U8 if color.dtype == torch.uint8 else PC_COLOR_F32
+    if thr is not None:
+        assert thr.dtype == torch.float32 and thr.numel() == 1 and thr.device == points.device
+    dev = points.device
+    ldp = (n + 3) // 4 * 4
+    mask = torch.empty(n, dtype=torch.uint8, device=dev)
+    planes = torch.empty((3, ldp), dtype=torch.float32, device=dev)
+    rgba = torch.empty(n, dtype=torch.int32, device=dev)
+    ws = torch.empty(_workspace("iggt_pointcloud_workspace", n), dtype=torch.uint8, device=dev)
+    _call(points, "iggt_pointcloud_select", 0, (21.0 + 3 * color.element_size()) * n, points.data_ptr(), conf.data_ptr(),
+          n, _ptr(thr), color.data_ptr(), kind, *geom, int(bg_flags), mask.data_ptr(), planes.data_ptr(), ldp,
+          rgba.data_ptr(), ws.data_ptr(), _STREAM)
+    return mask, planes[:, :n], rgba, ws
+
+
+def pointcloud_compact(points, mask, rgba, ws, count, minmax):
+    """The kept points of pointcloud_select in pixel order -> uint8 [16 n] holding xyz fp32 [m,3] then RGBA [m,4]
+    (the GLB point section; m is known on the device only).  count: a one-element int32 device tensor that receives m;
+    minmax: a six-element fp32 device tensor that receives the per-axis min, then max, NaNs left out."""
+    n = points.shape[0]
+    assert mask.shape == (n,) and rgba.shape == (n,) and count.numel() == 1 and minmax.numel() == 6
+    assert count.dtype == torch.int32 and minmax.dtype == torch.float32 and count.is_contiguous() and minmax.is_contiguous()
+    out = torch.empty(16 * n, dtype=torch.uint8, device=points.device)
+    _call(points, "iggt_pointcloud_compact", 0, 33.0 * n, points.data_ptr(), mask.data_ptr(), rgba.data_ptr(), n,
+          ws.data_ptr(), out.data_ptr(), count.data_ptr(), minmax.data_ptr(), _STREAM)
+    return out
 
 
 # ---------------------------------------------------------------------------------------------------

@@ -50,8 +50,14 @@ _JET_SEGMENTS = (
 
 def jet_lut(n=256):
     """[n, 3] float64: `jet` sampled at n evenly spaced points of [0, 1], piecewise linear between the segment rows."""
+    return segment_lut(_JET_SEGMENTS, n)
+
+
+def segment_lut(segments, n=256):
+    """[n, channels] float64: a matplotlib segment-data colormap ((x, y0, y1) rows per channel) sampled at n evenly
+    spaced points of [0, 1], as matplotlib builds its lookup table (gamma 1)."""
     out = []
-    for seg in _JET_SEGMENTS:
+    for seg in segments:
         a = np.asarray(seg, np.float64)
         x, y0, y1 = a[:, 0] * (n - 1), a[:, 1], a[:, 2]
         xs = (n - 1) * np.linspace(0.0, 1.0, n)

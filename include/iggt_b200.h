@@ -391,7 +391,8 @@ int iggt_quantile(const float* y, int64_t rows, int64_t n, int64_t ld, const flo
 
 /* The selection behind iggt_quantile, generalised (metrics.py:336 np.median, datasets/utils/misc.py:528-533
  * np.nanpercentile).  For every row r of y [rows, n] (row pitch ld), the values y[r, i] with mask[r, i] != 0 (mask
- * uint8 [rows, n], row pitch ldm; NULL = every value) are selected, and out [rows, nq] gets quantile q[i] of them under
+ * uint8 [rows, n], row pitch ldm, ldm = 0 shares one mask row between all rows; NULL = every value) are selected,
+ * and out [rows, nq] gets quantile q[i] of them under
  * `rule` (q a HOST array; for IGGT_QRULE_MEDIAN, q is ignored and nq = 1).  The target ranks are derived on the device
  * from each row's selected count, by the rank rule of iggt_quantile_rule; count [rows] int64 (may be NULL) receives
  * that count (NaNs left out under IGGT_QRULE_NUMPY_NAN).  An empty row gives NaN.  Bit for bit numpy 2.3 for float32
@@ -478,6 +479,37 @@ int iggt_depth_zero_outside(float* depth, int64_t S, int64_t n, const float* thr
  * ((u - cu) d / fu, (v - cv) d / fv, d) in fp64, one rounding per operation, rounded to fp32 (the reference's numpy
  * promotes the pixel grid and the intrinsics to float64).  intr [S, 3, 3] fp64. */
 int iggt_depth_to_cam(const float* depth, const double* intr, int S, int H, int W, float* cam, iggt_stream_t stream);
+
+/* ---- Point-cloud export (visual_util.py:38-238 predictions_to_glb, called three times per scene by demo.py:642;
+ * csrc/pointcloud.cu).  Points are fp32 [n, 3], 0 < n < 2^32, in pixel order. */
+
+#define IGGT_PC_COLOR_F32 0     /* colour source float32: (c * 255) rounded in fp32, then truncated to a byte */
+#define IGGT_PC_COLOR_U8 1      /* colour source uint8: c * 255 wraps mod 256 as numpy's uint8 product does */
+#define IGGT_PC_MASK_BLACK 1    /* drop points whose r + g + b < 16 (visual_util.py:184-186) */
+#define IGGT_PC_MASK_WHITE 2    /* drop points whose r, g and b are all > 240 (visual_util.py:188-192) */
+
+/* Host query: *bytes = device workspace size of iggt_pointcloud_select / iggt_pointcloud_compact for n points (the
+ * kept count of every tile of 1024 points, and its exclusive prefix). */
+int iggt_pointcloud_workspace(int64_t n, int64_t* bytes);
+
+/* One pass over n points (visual_util.py:167-192): keep point i where conf[i] >= *thr and conf[i] > float32(1e-5)
+ * (fp32 compares; thr is a DEVICE pointer, e.g. iggt_select's output, NULL = 0.0), and where the background masks in
+ * bg_flags (IGGT_PC_MASK_*) pass on its RGBA bytes.  Colour source of kind IGGT_PC_COLOR_*: channel c of point i at
+ * element (i / color_hw) * color_sf + c * color_sc + (i % color_hw) * color_sp (NCHW [S, 3, H, W]: hw = H W, sf = 3 H W,
+ * sc = H W, sp = 1; channels-last [n, 3]: hw = n, sf = 0, sc = 1, sp = 3).  Writes mask [n] uint8 (0 / 1), rgba [n]
+ * (r | g << 8 | b << 16 | 255 << 24), the coordinate planes [3, n] fp32 (row pitch ldp) for iggt_select with this mask
+ * and ldm = 0, and the tile counts into the workspace. */
+int iggt_pointcloud_select(const float* points, const float* conf, int64_t n, const float* thr, const void* color,
+                           int color_kind, int64_t color_hw, int64_t color_sf, int64_t color_sc, int64_t color_sp,
+                           int bg_flags, uint8_t* mask, float* planes, int64_t ldp, uint32_t* rgba, void* workspace,
+                           iggt_stream_t stream);
+
+/* The kept points of iggt_pointcloud_select (same n, mask, rgba and workspace), in pixel order (visual_util.py:194-195
+ * boolean indexing), as the GLB's point section: out = xyz fp32 [m, 3] followed by RGBA bytes [m, 4] (capacity 16 n
+ * bytes).  *count = m (device); minmax [6] fp32 (device) = per-axis min, then max, of the kept coordinates with NaNs
+ * left out (+inf / -inf where none is left; -0 orders below +0).  Deterministic: repeated calls give identical bytes. */
+int iggt_pointcloud_compact(const float* points, const uint8_t* mask, const uint32_t* rgba, int64_t n, void* workspace,
+                            void* out, uint32_t* count, float* minmax, iggt_stream_t stream);
 
 #ifdef __cplusplus
 }
