@@ -188,7 +188,8 @@ track_input_kernel(const float* __restrict__ coords, const float* __restrict__ f
     } else if (c < D) {
       x = tfeat[static_cast<int64_t>(row) * 128 + (c - 260)];
     }
-    if (c < D) x += pos[static_cast<int64_t>(bn) * D + c] + ref_tok[(s > 0 ? D : 0) + c];
+    // (x + pos) + ref in the reference's order (base_track_predictor.py:154, 160), so these fp32 sums match it bit for bit
+    if (c < D) x = (x + pos[static_cast<int64_t>(bn) * D + c]) + ref_tok[(s > 0 ? D : 0) + c];
     v[k] = x;
     sum += (c < D) ? x : 0.f;
     if (raw && c < D) raw[static_cast<int64_t>(row) * D + c] = x;

@@ -9,19 +9,19 @@ Bound 1 (per element):  |O - O64| <= ulp16(O64) + u_P * (P64 @ |V|) + 2^-20 * ma
     sums of O and l; and where an fp16 weight falls below 2^-14 it is subnormal, rounded to within 2^-25 absolute:
     over 1374 keys of random sign ~2^-25 * sqrt(1374 / 3) = 2^-20.6 of max|V|.
 The inputs scale q and k so that the logits have a standard deviation of about 8, which keeps the running max moving.
-The worst error / bound of each case is printed (run with -s to see it).
+The bound-1 check is `check_attn_bound1` in tests/ulp_bounds.py (tests/test_track_bounds_gpu.py applies it at the
+update transformer's shapes).  The worst error / bound of each case is printed (run with -s to see it).
 """
 import math
 
 import pytest
 import torch
 
-from ulp_bounds import check16, ulp16
+from ulp_bounds import check16, check_attn_bound1
 
 pytestmark = pytest.mark.gpu
 
 DTYPES = [torch.float16, torch.bfloat16]
-U_P = {torch.float16: 2.0 ** -11, torch.bfloat16: 2.0 ** -8}
 
 
 @pytest.fixture(scope="module")
@@ -36,35 +36,6 @@ def _splits(Lk, want):
     s = min(want, n_kv)
     tps = (n_kv + s - 1) // s
     return (n_kv + tps - 1) // tps
-
-
-def _attn64(q, k, v, num_seq, Lq, Lk, H, scale):
-    """O64 = softmax(q k^T * scale) v per sequence and head in float64, P64 @ |V|, and max|V| per (sequence, head),
-    all as [num_seq * Lq, H * 64]."""
-    q4 = q.double().reshape(num_seq, Lq, H, 64).transpose(1, 2)
-    k4 = k.double().reshape(num_seq, Lk, H, 64).transpose(1, 2)
-    v4 = v.double().reshape(num_seq, Lk, H, 64).transpose(1, 2)
-    p = torch.softmax(q4 @ k4.transpose(-1, -2) * scale, -1)
-    vmax = v4.abs().amax(dim=(2, 3), keepdim=True).expand(num_seq, H, Lq, 64)
-
-    def flat(t):
-        return t.transpose(1, 2).reshape(num_seq * Lq, H * 64)
-
-    return flat(p @ v4), flat(p @ v4.abs()), flat(vmax)
-
-
-def _check_bound1(out, q, k, v, num_seq, Lq, Lk, H, dtype, scale=0.125, what=""):
-    o64, pv, vmax = _attn64(q, k, v, num_seq, Lq, Lk, H, scale)
-    bound = ulp16(o64, dtype) + U_P[dtype] * pv + 2.0 ** -20 * vmax
-    o = out.double()
-    assert torch.isfinite(o).all(), f"{what}: non-finite outputs"
-    ratio = ((o - o64).abs() / bound)
-    worst = ratio.max().item()
-    i = int(ratio.view(-1).argmax())
-    assert worst <= 1.0, (f"{what}: {int((ratio > 1).sum())} of {o.numel()} elements beyond bound 1; worst "
-                          f"{worst:.3g} x bound at {divmod(i, o.shape[1])}: out {o.view(-1)[i].item()!r} "
-                          f"ref {o64.view(-1)[i].item()!r}")
-    return worst
 
 
 def _qkv(g, num_seq, Lq, Lk, H, dtype, logit_std=8.0):
@@ -96,7 +67,7 @@ def test_bound_vs_fp64_softmax(ops, dtype, split, Lk):
             s = _splits(Lk, 3) if split else 1
             out = ops.attention(q, k, v, num_seq, Lq, Lk, H, splits=s)
             torch.cuda.synchronize()
-            worst = max(worst, _check_bound1(out, q, k, v, num_seq, Lq, Lk, H, dtype,
+            worst = max(worst, check_attn_bound1(out, q, k, v, num_seq, Lq, Lk, H, dtype,
                                              what=f"num_seq={num_seq} Lq={Lq} Lk={Lk} splits={s}"))
     _report(f"attention bound1 {dtype} Lk={Lk} split={split}", worst)
 
@@ -188,7 +159,7 @@ def test_poisoned_neighbour(ops, dtype, split, Lk):
     out = ops.attention(q, k, v, num_seq, Lq, Lk, H, splits=s)
     torch.cuda.synchronize()
     _report(f"poisoned neighbour {dtype} Lk={Lk} splits={s}",
-            _check_bound1(out, q, k, v, num_seq, Lq, Lk, H, dtype, what=f"poisoned Lk={Lk} splits={s}"))
+            check_attn_bound1(out, q, k, v, num_seq, Lq, Lk, H, dtype, what=f"poisoned Lk={Lk} splits={s}"))
 
 
 # -------------------------------------------------------------------------------------------- 5. non-finite isolation
@@ -233,4 +204,4 @@ def test_packed_qkv_slices(ops, dtype, num_seq, L, H):
     torch.cuda.synchronize()
     assert torch.equal(out, ref_bits)
     _report(f"packed qkv {dtype} {num_seq}x{L} H={H}",
-            _check_bound1(out, q, k, v, num_seq, L, L, H, dtype, what=f"packed qkv {num_seq}x{L}"))
+            check_attn_bound1(out, q, k, v, num_seq, L, L, H, dtype, what=f"packed qkv {num_seq}x{L}"))

@@ -127,3 +127,38 @@ def check32(out, ref64, scale64, rel, lo64=None, hi64=None, what=""):
                         f"{_where(i, out.shape)}: out {o.reshape(-1)[i].item()!r} ref {ref64.reshape(-1)[i].item()!r} "
                         f"scale {scale64.reshape(-1)[i].item()!r} ({worst:.3g} x bound)")
     return worst
+
+
+# ------------------------------------------------------------------------------------------- flash attention, bound 1
+# |O - O64| <= ulp16(O64) + u_P * (P64 @ |V|) + 2^-20 * max|V| per element, derived in tests/test_attention_bounds_gpu.py
+U_P = {torch.float16: 2.0 ** -11, torch.bfloat16: 2.0 ** -8}     # P is rounded to 16 bit before P V
+
+
+def attn64(q, k, v, num_seq, Lq, Lk, H, scale):
+    """O64 = softmax(q k^T * scale) v per sequence and head in float64, P64 @ |V|, and max|V| per (sequence, head),
+    all as [num_seq * Lq, H * 64]."""
+    q4 = q.double().reshape(num_seq, Lq, H, 64).transpose(1, 2)
+    k4 = k.double().reshape(num_seq, Lk, H, 64).transpose(1, 2)
+    v4 = v.double().reshape(num_seq, Lk, H, 64).transpose(1, 2)
+    p = torch.softmax(q4 @ k4.transpose(-1, -2) * scale, -1)
+    vmax = v4.abs().amax(dim=(2, 3), keepdim=True).expand(num_seq, H, Lq, 64)
+
+    def flat(t):
+        return t.transpose(1, 2).reshape(num_seq * Lq, H * 64)
+
+    return flat(p @ v4), flat(p @ v4.abs()), flat(vmax)
+
+
+def check_attn_bound1(out, q, k, v, num_seq, Lq, Lk, H, dtype, scale=0.125, what=""):
+    """Asserts bound 1 on every element of the attention output; returns the worst error / bound."""
+    o64, pv, vmax = attn64(q, k, v, num_seq, Lq, Lk, H, scale)
+    bound = ulp16(o64, dtype) + U_P[dtype] * pv + 2.0 ** -20 * vmax
+    o = out.double()
+    assert torch.isfinite(o).all(), f"{what}: non-finite outputs"
+    ratio = ((o - o64).abs() / bound)
+    worst = ratio.max().item()
+    i = int(ratio.view(-1).argmax())
+    assert worst <= 1.0, (f"{what}: {int((ratio > 1).sum())} of {o.numel()} elements beyond bound 1; worst "
+                          f"{worst:.3g} x bound at {divmod(i, o.shape[1])}: out {o.view(-1)[i].item()!r} "
+                          f"ref {o64.view(-1)[i].item()!r}")
+    return worst
