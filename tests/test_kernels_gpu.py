@@ -112,65 +112,6 @@ def test_gemm_store32(ops, dtype):
     assert _relmax(out, ref) < 2e-5
 
 
-def _rope_tables(npos, device):
-    # iggt/layers/rope.py:103-112 with feature_dim 32, base 100
-    exponents = torch.arange(0, 32, 2, device=device).float() / 32
-    inv_freq = 1.0 / (100.0 ** exponents)
-    ang = torch.einsum("i,j->ij", torch.arange(npos, device=device, dtype=torch.float32), inv_freq)
-    return ang.cos().contiguous(), ang.sin().contiguous()
-
-
-def _rope_ref(t, pos):
-    # t [M, H, 64] fp32, pos [M, 2] long (y, x)  -- iggt/layers/rope.py:119-188
-    cos16, sin16 = _rope_tables(int(pos.max()) + 1, t.device)
-    cos = torch.cat([cos16, cos16], -1)
-    sin = torch.cat([sin16, sin16], -1)
-
-    def rot(x):
-        return torch.cat([-x[..., 16:], x[..., :16]], -1)
-
-    def one(x, p):
-        c, s = cos[p][:, None, :], sin[p][:, None, :]
-        return x * c + rot(x) * s
-
-    return torch.cat([one(t[..., :32], pos[:, 0]), one(t[..., 32:], pos[:, 1])], -1)
-
-
-@pytest.mark.parametrize("dtype", DTYPES)
-@pytest.mark.parametrize("qk_norm", [False, True])
-@pytest.mark.parametrize("gh,gw,S", [(5, 7, 3), (13, 16, 5)])      # 1 row tile / 9 row tiles (CTA pairs)
-def test_gemm_qkv(ops, dtype, qk_norm, gh, gw, S):
-    C, K = 1024, 1024
-    T = 5 + gh * gw
-    M = S * T
-    g = torch.Generator(device="cuda").manual_seed(3)
-    a = torch.randn(M, K, device="cuda", generator=g).to(dtype)
-    w = (torch.randn(3 * C, K, device="cuda", generator=g) / math.sqrt(K)).to(dtype)
-    bias = torch.randn(3 * C, device="cuda", generator=g) * 0.1
-    qn_w = torch.rand(64, device="cuda", generator=g) + 0.5
-    qn_b = torch.randn(64, device="cuda", generator=g) * 0.1
-    kn_w = torch.rand(64, device="cuda", generator=g) + 0.5
-    kn_b = torch.randn(64, device="cuda", generator=g) * 0.1
-    yy, xx = torch.meshgrid(torch.arange(gh, device="cuda"), torch.arange(gw, device="cuda"), indexing="ij")
-    pos = torch.cat([torch.zeros(5, 2, dtype=torch.long, device="cuda"),
-                     torch.stack([yy.reshape(-1), xx.reshape(-1)], -1) + 1], 0)  # [T,2]
-    cos, sin = _rope_tables(max(gh, gw) + 1, "cuda")
-    out = ops.gemm_qkv(a, w, bias, C, qk_norm=qk_norm, qn_w=qn_w, qn_b=qn_b, kn_w=kn_w, kn_b=kn_b,
-                       rope_cos=cos, rope_sin=sin, pos_yx=pos.int().contiguous(), T=T)
-    torch.cuda.synchronize()
-    ref = (a.float() @ w.float().t() + bias)
-    if qk_norm:
-        ref = ref.to(dtype).float()  # the autocast Linear output is 16-bit before the fp32 LayerNorm
-        q, k, v = ref.view(M, 3, 16, 64).unbind(1)
-        q = F.layer_norm(q, (64,), qn_w, qn_b, 1e-5)
-        k = F.layer_norm(k, (64,), kn_w, kn_b, 1e-5)
-        posm = pos.repeat(S, 1)
-        q, k = _rope_ref(q, posm), _rope_ref(k, posm)
-        ref = torch.stack([q, k, v], 1).reshape(M, 3 * C)
-    # LayerNorm(64) amplifies a 16-bit rounding flip of its input by ~1/std, so allow 4 ulp
-    assert _relmax(out, ref) < 4 * _tol(dtype)
-
-
 @pytest.mark.parametrize("dtype", DTYPES)
 @pytest.mark.parametrize("num_seq,Lq,Lk,H", [(3, 300, 300, 4), (2, 1374, 1374, 16), (1, 200, 900, 2), (1, 128, 128, 1)])
 def test_attention(ops, dtype, num_seq, Lq, Lk, H):
