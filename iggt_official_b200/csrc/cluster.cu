@@ -24,6 +24,7 @@
 #include <cmath>
 #include <vector>
 
+#include "launch.cuh"
 #include "../../include/iggt_b200.h"
 
 namespace iggt {
@@ -510,12 +511,11 @@ extern "C" int iggt_cluster_core(const float* sorted8, const float* box, int64_t
                                  iggt_stream_t stream) {
   if (!sorted8 || !box || !core2 || n <= 0 || n >= (1LL << 31) || k < 1 || k > CL_KMAX || k >= n) return -1;
   const size_t smem = static_cast<size_t>(k) * CL_CTA * sizeof(float);
-  static bool attr = false;
-  if (!attr) {
+  static DeviceOnce once;                               // the opt-in holds for the current device only
+  if (once.first()) {
     const cudaError_t e = cudaFuncSetAttribute(cl_core_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                                CL_KMAX * CL_CTA * static_cast<int>(sizeof(float)));
-    if (e != cudaSuccess) return (int)e;
-    attr = true;
+    if (e != cudaSuccess) { once.reset_current(); return (int)e; }
   }
   const int nb = static_cast<int>((n + CL_TILE - 1) / CL_TILE);
   cl_core_kernel<<<static_cast<unsigned>((n + CL_CTA - 1) / CL_CTA), CL_CTA, smem, (cudaStream_t)stream>>>(

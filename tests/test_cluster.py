@@ -193,7 +193,8 @@ def _prep(x):
 @pytest.mark.gpu
 @pytest.mark.parametrize("kind,n,k", [("random", 5000, 1), ("random", 5000, 100), ("clustered", 20000, 100),
                                       ("clustered", 6000, 256), ("duplicates", 3000, 100), ("duplicates", 3000, 1),
-                                      ("random", 700, 256), ("random", 300, 7)])
+                                      ("random", 700, 256), ("random", 300, 7), ("random", 1500, 512),
+                                      ("clustered", 4097, 511)])
 def test_device_core_distances(kind, n, k):
     from scipy.spatial import cKDTree
     from iggt_official_b200 import ops
