@@ -19,24 +19,22 @@ twice those.
 
 The worst value of each check (ulps, share off RN, error / bound) is printed, so a run with -s reports the margins.
 """
-import ctypes
 import math
 
 import pytest
 import torch
 import torch.nn.functional as F
 
+from launch_refs import ACC, FRAC, FRAC_GELU, GELU_ERR
+from launch_refs import act_interval as _act_interval
+from launch_refs import gelu64 as _gelu64
+from launch_refs import gemm64 as _gemm64
+from launch_refs import gemm_plan as _plan
 from ulp_bounds import around, check16, check32, rn16, ulp16
 
 pytestmark = pytest.mark.gpu
 
 DTYPES = [torch.float16, torch.bfloat16]
-ACC = 2.0 ** -20
-# gelu_fast (csrc/ptx.cuh): Abramowitz-Stegun erf (|err| <= 1.5e-7), the fp32 complement 1 - erf (quantised at
-# 2^-24) and ex2.approx (2^-22 relative), each scaled by |x| / 2
-GELU_ERR = 1.5e-7 + 2.0 ** -24 + 2.0 ** -22
-FRAC = {torch.float16: 0.01, torch.bfloat16: 0.002}
-FRAC_GELU = {torch.float16: 0.02, torch.bfloat16: 0.005}
 
 
 @pytest.fixture(scope="module")
@@ -49,14 +47,6 @@ def _report(what, value):
     print(f"[bound] {what}: {value}")
 
 
-def _gelu64(x):
-    return 0.5 * x * (1.0 + torch.erf(x / math.sqrt(2.0)))
-
-
-def _leaky64(x):
-    return torch.where(x > 0, x, 0.01 * x)
-
-
 def _operands(g, M, N, K, dtype, lda_pad=0, ldw_pad=0):
     """A [M,K] and W [N,K] 16-bit, as column slices of wider tensors when a pad is given (offset 8 columns: TMA wants
     16-byte aligned bases)."""
@@ -65,32 +55,6 @@ def _operands(g, M, N, K, dtype, lda_pad=0, ldw_pad=0):
     a = a_full[:, 8:8 + K] if lda_pad else a_full
     w = w_full[:, 8:8 + K] if ldw_pad else w_full
     return a, w
-
-
-def _gemm64(a, w):
-    """Exact (fp64) product of the 16-bit operands and its per-element magnitude sum."""
-    a64, w64 = a.double(), w.double()
-    return a64 @ w64.t(), a64.abs() @ w64.abs().t()
-
-
-def _plan(M, N, K, epi=1):
-    from iggt_official_b200 import _lib
-    out = (ctypes.c_int * 7)()
-    assert _lib.load().iggt_gemm_plan(epi, M, N, K, ctypes.cast(out, ctypes.c_void_p)) == 0
-    return dict(zip(["bn", "pair", "stream_k", "m_tiles", "n_tiles", "k_blocks", "grid"], list(out)))
-
-
-def _act_interval(act, y, s, dtype):
-    """(ref, lo, hi) of act(y) when the kernel's fp32 value lies within y -+ s.  act 1 is the autocast form: GELU of the
-    16-bit Linear output (gemm.cuh: round16 before gelu_fast2), with the gelu_fast error on top."""
-    lo, hi = around(y, s)
-    if act == 1:
-        x_lo, x_hi = rn16(lo, dtype).double(), rn16(hi, dtype).double()
-        g_lo, g_hi = _gelu64(x_lo), _gelu64(x_hi)
-        e = torch.maximum(x_lo.abs(), x_hi.abs()) / 2 * GELU_ERR
-        return _gelu64(rn16(y, dtype).double()), torch.minimum(g_lo, g_hi) - e, torch.maximum(g_lo, g_hi) + e
-    f = {0: lambda t: t, 2: torch.relu, 3: _leaky64}[act]
-    return f(y), f(lo), f(hi)
 
 
 # --------------------------------------------------------------------------------------------- 1. shapes and strides

@@ -20,12 +20,15 @@ import pytest
 import torch
 import torch.nn.functional as F
 
+from launch_refs import U24
+from launch_refs import check_tail as _check_tail
+from launch_refs import conf64 as _conf64
+from launch_refs import tail_act64 as _tail_act64
 from ulp_bounds import check16, check32, ulp16, ulp_distance
 
 pytestmark = pytest.mark.gpu
 
 DTYPES = [torch.float16, torch.bfloat16]
-U24 = 2.0 ** -24
 U_SPLIT_P = {torch.float16: 2.0 ** -22, torch.bfloat16: 2.0 ** -16}      # what the hi + lo split of P leaves
 
 
@@ -298,36 +301,6 @@ def test_upsample_bilinear_edges(ops, dtype, h, w, H, W, with_pe):
 
 
 # ------------------------------------------------------------------------------------------------- dpt tails (fp32 out)
-def _tail_act64(o64, A, mode, rel):
-    """Reference and bound of the head activation of o (exact o64, |o - o64| <= rel A):
-      exp(o):           |d| <= e^o (e^(rel A) - 1) + expf's 2^-22 e^o
-      sign expm1(|o|):  |d| <= e^|o| (e^(rel A) - 1) + expm1f's 2^-22 |expm1|
-      1 + exp(o):       as exp, + the add's 2^-24 (1 + e^o)
-    returned as (ref, scale) for check32(out, ref, scale, rel): the bound is rel * scale."""
-    grow = torch.expm1(rel * A) / rel                       # (e^(rel A) - 1) / rel  (~A)
-    if mode == 0:
-        e = torch.exp(o64)
-        return e, e * (grow + 2.0 ** -22 / rel)
-    r = torch.sign(o64) * torch.expm1(o64.abs())
-    return r, torch.exp(o64.abs()) * grow + r.abs() * 2.0 ** -22 / rel
-
-
-def _conf64(o64, A, rel):
-    e = torch.exp(o64)
-    return 1 + e, e * (torch.expm1(rel * A) / rel + 2.0 ** -22 / rel) + (1 + e) * U24 / rel
-
-
-def _check_tail(main, conf, o64, A, mode, rel, what):
-    """o64 / A: [NB, H, W, OC] exact pre-activation and its magnitude sum."""
-    if mode == 2:                                  # part features: channels-first, no confidence
-        assert conf is None
-        return check32(main, o64.permute(0, 3, 1, 2), A.permute(0, 3, 1, 2), rel, what=what)
-    ref, scale = _tail_act64(o64[..., :-1], A[..., :-1], mode, rel)
-    w1 = check32(main, ref, scale, rel, what=what)
-    cref, cscale = _conf64(o64[..., -1], A[..., -1], rel)
-    return max(w1, check32(conf, cref, cscale, rel, what=what + " conf"))
-
-
 TAIL_SHAPES = [(2, 37, 50), (1, 16, 8), (3, 5, 3), (1, 100, 131), (1, 518, 518)]
 
 

@@ -26,23 +26,6 @@ def ops():
     return _ops
 
 
-@pytest.mark.parametrize("dtype", DTYPES)
-@pytest.mark.parametrize("M,N,K,act", [(300, 320, 192, 0), (2748, 4096, 1024, 1), (128, 64, 64, 2), (77, 32, 128, 3),
-                                        (1000, 768, 2048, 0),
-                                        (1102, 4096, 256, 1)])   # 9 row tiles, the last one partly filled
-def test_gemm_store16(ops, dtype, M, N, K, act):
-    g = torch.Generator(device="cuda").manual_seed(M + N + K)
-    a = torch.randn(M, K, device="cuda", generator=g).to(dtype)
-    w = (torch.randn(N, K, device="cuda", generator=g) / math.sqrt(K)).to(dtype)
-    bias = torch.randn(N, device="cuda", generator=g)
-    ref = a.float() @ w.float().t() + bias
-    ref = {0: lambda t: t, 1: lambda t: F.gelu(t), 2: F.relu, 3: lambda t: F.leaky_relu(t, 0.01)}[act](ref)
-    out = ops.gemm_store16(a, w, bias, act=act)
-    torch.cuda.synchronize()
-    assert out.shape == (M, N)
-    assert _relmax(out, ref) < 2 * _tol(dtype)
-
-
 def test_relu_epilogues_keep_nan_like_torch(ops):
     """torch.relu(nan) = nan, relu(-inf) = 0, relu(inf) = inf: an overflowed fp16 head activation must stay visible through
     the ReLU epilogues (fmaxf would turn inf - inf into 0 and hand `check_finite` finite garbage)."""
@@ -68,138 +51,10 @@ def test_relu_epilogues_keep_nan_like_torch(ops):
     assert torch.isnan(y[0, 2:5, 2:5]).all() and torch.isfinite(y[0, 6:, 6:]).all()
 
 
-@pytest.mark.parametrize("dtype", DTYPES)
-def test_gemm_store16_addend(ops, dtype):
-    M, N, K, R = 3 * 361, 256, 2048, 361
-    g = torch.Generator(device="cuda").manual_seed(5)
-    a = torch.randn(M, K, device="cuda", generator=g).to(dtype)
-    w = (torch.randn(N, K, device="cuda", generator=g) / math.sqrt(K)).to(dtype)
-    bias = torch.randn(N, device="cuda", generator=g)
-    add = torch.randn(R, N, device="cuda", generator=g).to(dtype)
-    ref = a.float() @ w.float().t() + bias + add.float().repeat(3, 1)
-    out = ops.gemm_store16(a, w, bias, addend=add, add_rows=R)
-    torch.cuda.synchronize()
-    assert _relmax(out, ref) < 2 * _tol(dtype)
-
-
-@pytest.mark.parametrize("dtype", DTYPES)
-@pytest.mark.parametrize("M,N,K", [(300, 1024, 1024), (2748, 1024, 4096), (9, 2048, 2048),
-                                   (1102, 2048, 512)])            # stream-K over CTA pairs, odd row-tile count
-def test_gemm_resid32(ops, dtype, M, N, K):
-    g = torch.Generator(device="cuda").manual_seed(1)
-    a = torch.randn(M, K, device="cuda", generator=g).to(dtype)
-    w = (torch.randn(N, K, device="cuda", generator=g) / math.sqrt(K)).to(dtype)
-    bias = torch.randn(N, device="cuda", generator=g)
-    gamma = torch.rand(N, device="cuda", generator=g) + 0.5
-    x = torch.randn(M, N, device="cuda", generator=g)
-    ref = x + gamma * (a.float() @ w.float().t() + bias)
-    ops.gemm_resid32(a, w, x, bias, gamma)
-    torch.cuda.synchronize()
-    # fp32 output: only accumulation-order noise (K products of 16-bit values)
-    assert _relmax(x, ref) < 2e-5
-
-
-@pytest.mark.parametrize("dtype", DTYPES)
-def test_gemm_store32(ops, dtype):
-    M, N, K = 137, 520, 256
-    g = torch.Generator(device="cuda").manual_seed(2)
-    a = torch.randn(M, K, device="cuda", generator=g).to(dtype)
-    w = (torch.randn(N, K, device="cuda", generator=g) / math.sqrt(K)).to(dtype)
-    bias = torch.randn(N, device="cuda", generator=g)
-    ref = a.float() @ w.float().t() + bias
-    out = ops.gemm_store32(a, w, bias)
-    torch.cuda.synchronize()
-    assert _relmax(out, ref) < 2e-5
-
-
-@pytest.mark.parametrize("dtype", DTYPES)
-@pytest.mark.parametrize("num_seq,Lq,Lk,H", [(3, 300, 300, 4), (2, 1374, 1374, 16), (1, 200, 900, 2), (1, 128, 128, 1)])
-def test_attention(ops, dtype, num_seq, Lq, Lk, H):
-    g = torch.Generator(device="cuda").manual_seed(7)
-    C = H * 64
-    qkv_q = torch.randn(num_seq * Lq, C, device="cuda", generator=g).to(dtype)
-    kv = torch.randn(num_seq * Lk, 2 * C, device="cuda", generator=g).to(dtype)
-    k, v = kv[:, :C], kv[:, C:]
-    out = ops.attention(qkv_q, k, v, num_seq, Lq, Lk, H)
-    torch.cuda.synchronize()
-    q4 = qkv_q.float().view(num_seq, Lq, H, 64).transpose(1, 2)
-    k4 = k.float().reshape(num_seq, Lk, H, 64).transpose(1, 2)
-    v4 = v.float().reshape(num_seq, Lk, H, 64).transpose(1, 2)
-    att = torch.softmax(q4 @ k4.transpose(-1, -2) * 0.125, -1) @ v4
-    ref = att.transpose(1, 2).reshape(num_seq * Lq, C)
-    # P is rounded to 16 bit before PV (as in every flash kernel): 2 ulp of the output scale
-    assert _relmax(out, ref) < 3 * _tol(dtype)
-
-@pytest.mark.parametrize("dtype", [torch.float16, torch.bfloat16])
-@pytest.mark.parametrize("num_seq,Lq,Lk,H,splits", [(1, 1374, 10992, 16, 3), (1, 1374, 10992, 16, 5), (2, 300, 1000, 4, 2),
-                                                    (1, 129, 257, 2, 3), (3, 64, 700, 1, 6), (1, 2748, 10992, 16, 2)])
-def test_attention_split_kv(ops, dtype, num_seq, Lq, Lk, H, splits):
-    """Split-KV launches (view-sharded ranks): every (item, kv range) writes un-normalised O and (m, l) to the workspace,
-    the merge kernel combines them - must equal the exact softmax and the unsplit launch."""
-    g = torch.Generator(device="cuda").manual_seed(11)
-    C = H * 64
-    q = torch.randn(num_seq * Lq, C, device="cuda", generator=g).to(dtype)
-    kv = torch.randn(num_seq * Lk, 2 * C, device="cuda", generator=g).to(dtype)
-    kv[: Lk // 3] *= 4.0                                   # the running max of the first range is not the global one
-    k, v = kv[:, :C], kv[:, C:]
-    out = ops.attention(q, k, v, num_seq, Lq, Lk, H, splits=splits)
-    one = ops.attention(q, k, v, num_seq, Lq, Lk, H, splits=1)
-    torch.cuda.synchronize()
-    q4 = q.float().view(num_seq, Lq, H, 64).transpose(1, 2)
-    k4 = k.float().reshape(num_seq, Lk, H, 64).transpose(1, 2)
-    v4 = v.float().reshape(num_seq, Lk, H, 64).transpose(1, 2)
-    ref = (torch.softmax(q4 @ k4.transpose(-1, -2) * 0.125, -1) @ v4).transpose(1, 2).reshape(num_seq * Lq, C)
-    assert _relmax(out, ref) < 3 * _tol(dtype)
-    assert _relmax(out, one.float()) < 2 * _tol(dtype)
-
-
 def test_attention_plan_is_used_and_cached(ops):
     s, ws = ops.attention_plan(1, 1374, 10992, 16)
     assert s >= 1 and (ws > 0) == (s > 1) and ops.attention_plan(1, 1374, 10992, 16) == (s, ws)
     assert ops.attention_plan(8, 1374, 1374, 16)[0] == 1
-
-
-@pytest.mark.parametrize("out_dtype", [torch.float16, torch.bfloat16, torch.float32])
-@pytest.mark.parametrize("C", [1024, 2048])
-def test_layernorm(ops, out_dtype, C):
-    g = torch.Generator(device="cuda").manual_seed(9)
-    G, rin, off, rout = 3, 50, 5, 45
-    x = torch.randn(G * rin, C, device="cuda", generator=g) * 3 + 1
-    w = torch.rand(C, device="cuda", generator=g) + 0.5
-    b = torch.randn(C, device="cuda", generator=g)
-    out = torch.zeros(G * rout, C, device="cuda", dtype=out_dtype)
-    ops.layernorm(x, w, b, 1e-6, out, groups=G, rows_out=rout, rows_in=rin, in_off=off)
-    torch.cuda.synchronize()
-    ref = F.layer_norm(x.view(G, rin, C)[:, off:off + rout].reshape(-1, C), (C,), w, b, 1e-6)
-    tol = 1e-5 if out_dtype == torch.float32 else _tol(out_dtype)
-    assert _relmax(out, ref) < tol
-
-
-@pytest.mark.parametrize("dtype", DTYPES)
-@pytest.mark.parametrize("NB,H,W,Cin,Cout,taps,act,use_res", [(2, 37, 37, 256, 256, 9, 2, True), (1, 20, 50, 64, 128, 9, 0, False),
-                                                              (2, 19, 19, 1024, 256, 9, 0, False), (1, 30, 30, 128, 32, 9, 2, False),
-                                                              (2, 37, 37, 256, 256, 1, 0, False),
-                                                              # 143 spatial tiles x 256 channels: CTA pairs, odd count
-                                                              (1, 88, 208, 64, 256, 9, 2, True),
-                                                              (1, 88, 208, 64, 256, 1, 0, False)])
-def test_conv_nhwc(ops, dtype, NB, H, W, Cin, Cout, taps, act, use_res):
-    g = torch.Generator(device="cuda").manual_seed(11)
-    x = torch.randn(NB, H, W, Cin, device="cuda", generator=g).to(dtype)
-    ks = 3 if taps == 9 else 1
-    w = (torch.randn(Cout, Cin, ks, ks, device="cuda", generator=g) / math.sqrt(Cin * taps)).to(dtype)
-    bias = torch.randn(Cout, device="cuda", generator=g)
-    res = torch.randn(NB, H, W, Cout, device="cuda", generator=g).to(dtype) if use_res else None
-    wp = w.permute(0, 2, 3, 1).reshape(Cout, taps * Cin).contiguous()
-    out = ops.conv_nhwc(x, wp, bias, act=act, resid=res, taps=taps)
-    torch.cuda.synchronize()
-    torch.backends.cudnn.allow_tf32 = False
-    ref = F.conv2d(x.float().permute(0, 3, 1, 2), w.float(), bias, padding=ks // 2)
-    if act == 2:
-        ref = F.relu(ref)
-    ref = ref.permute(0, 2, 3, 1)
-    if use_res:
-        ref = ref + res.float()
-    assert _relmax(out, ref) < 2 * _tol(dtype)
 
 
 @pytest.mark.parametrize("dtype", DTYPES)

@@ -60,13 +60,16 @@ import math
 import pytest
 import torch
 
+from launch_refs import ACC
+from launch_refs import ln64 as _ln64
+from launch_refs import qk64 as _qk64
+from launch_refs import rope64 as _rope64
+from launch_refs import y64 as _y64
 from ulp_bounds import check16, check_attn_bound1, rn16
 
 pytestmark = pytest.mark.gpu
 
 DTYPES = [torch.float16, torch.bfloat16]
-ACC = 2.0 ** -20
-EPS = 1e-5
 NUM_SPECIAL = 5                       # camera + 4 register tokens per view, RoPE position (0, 0)
 NAN_ROWS = 3                          # NaN rows appended to the RoPE tables: a read past the valid rows shows
 SENTINEL = -1                         # 0xFFFF: a NaN pattern the kernel's round-to-nearest stores never produce
@@ -135,55 +138,6 @@ def _gauss_operands(g, M, C, K, dtype):
     w = (torch.randn(3 * C, K, device="cuda", generator=g) / math.sqrt(K)).to(dtype)
     bias = torch.randn(3 * C, device="cuda", generator=g).to(dtype).float()
     return a, w, bias
-
-
-def _y64(a, w, bias):
-    """acc + b in float64 from the 16-bit operands, and the magnitude sum |A| |W|^T + |b|."""
-    a64, w64, b64 = a.double(), w.double(), bias.double()
-    return a64 @ w64.t() + b64, a64.abs() @ w64.abs().t() + b64.abs()
-
-
-def _ln64(x, C, norm, amb=None):
-    """LayerNorm(64) of every q and k head of x [M, 2C] (the 16-bit Linear output as float64), two-pass, with the q
-    vectors on [0, C) and the k vectors on [C, 2C); returns (ln, slack), the slack of the module docstring, widened by
-    2 x the first-order effect of the ambiguous inputs `amb` (a_j per element, 0 where not ambiguous) when given."""
-    M, H = x.shape[0], C // 64
-    x = x.reshape(M, 2, H, 64)
-    w = torch.stack([norm[0], norm[2]]).double().view(1, 2, 1, 64)
-    b = torch.stack([norm[1], norm[3]]).double().view(1, 2, 1, 64)
-    mean = x.mean(-1, keepdim=True)
-    d = x - mean
-    rstd = (d.square().mean(-1, keepdim=True) + EPS).rsqrt()
-    z = d * rstd
-    zw = z * w
-    ln = zw + b
-    s = 2.0 ** -18 * rstd * w.abs() * x.abs().mean(-1, keepdim=True) + 2.0 ** -17 * zw.abs() + 2.0 ** -23 * ln.abs()
-    if amb is not None:
-        a = amb.reshape(M, 2, H, 64)
-        za = z.abs()
-        first = rstd * w.abs() * (a + (a.sum(-1, keepdim=True) + za * (a * za).sum(-1, keepdim=True)) / 64)
-        s = s + 2.0 * first
-    return ln.reshape(M, 2 * C), s.reshape(M, 2 * C)
-
-
-def _rope64(ln, s, cos, sin, pos, T):
-    """2-D RoPE of ln [M, 2C] at pos[row % T] with the fp32 table values, and the slack carried through it."""
-    M = ln.shape[0]
-    p = pos.long()[torch.arange(M, device=ln.device) % T]                  # [M, 2]: (y, x)
-    c = cos.double()[p].view(M, 1, 2, 16)                                  # half 0 rotates by y, half 1 by x
-    sn = sin.double()[p].view(M, 1, 2, 16)
-    l4, s4 = ln.view(M, -1, 2, 32), s.view(M, -1, 2, 32)
-    a, b = l4[..., :16], l4[..., 16:]
-    sa, sb = s4[..., :16], s4[..., 16:]
-    oa, ob = a * c - b * sn, b * c + a * sn
-    ea = c.abs() * sa + sn.abs() * sb + 2.0 ** -23 * ((a * c).abs() + (b * sn).abs() + oa.abs())
-    eb = c.abs() * sb + sn.abs() * sa + 2.0 ** -23 * ((b * c).abs() + (a * sn).abs() + ob.abs())
-    return torch.cat([oa, ob], -1).reshape(M, -1), torch.cat([ea, eb], -1).reshape(M, -1)
-
-
-def _qk64(u, C, T, norm, cos, sin, pos, amb=None):
-    ln, s = _ln64(u[:, :2 * C], C, norm, None if amb is None else amb[:, :2 * C])
-    return _rope64(ln, s, cos, sin, pos, T)
 
 
 def _check(out, ref, slack, dtype, frac, what):

@@ -134,31 +134,36 @@ def check32(out, ref64, scale64, rel, lo64=None, hi64=None, what=""):
 U_P = {torch.float16: 2.0 ** -11, torch.bfloat16: 2.0 ** -8}     # P is rounded to 16 bit before P V
 
 
-def attn64(q, k, v, num_seq, Lq, Lk, H, scale):
-    """O64 = softmax(q k^T * scale) v per sequence and head in float64, P64 @ |V|, and max|V| per (sequence, head),
-    all as [num_seq * Lq, H * 64]."""
-    q4 = q.double().reshape(num_seq, Lq, H, 64).transpose(1, 2)
-    k4 = k.double().reshape(num_seq, Lk, H, 64).transpose(1, 2)
-    v4 = v.double().reshape(num_seq, Lk, H, 64).transpose(1, 2)
-    p = torch.softmax(q4 @ k4.transpose(-1, -2) * scale, -1)
-    vmax = v4.abs().amax(dim=(2, 3), keepdim=True).expand(num_seq, H, Lq, 64)
-
-    def flat(t):
-        return t.transpose(1, 2).reshape(num_seq * Lq, H * 64)
-
-    return flat(p @ v4), flat(p @ v4.abs()), flat(vmax)
+def attn64(q, k, v, Lk, scale):
+    """One head of one sequence in float64: q [Lq, 64], k / v [Lk, 64] -> O64 = softmax(q k^T * scale) v and P64 @ |V|."""
+    k64, v64 = k.double(), v.double()
+    p = torch.softmax(q.double() @ k64.t() * scale, -1)
+    return p @ v64, p @ v64.abs()
 
 
-def check_attn_bound1(out, q, k, v, num_seq, Lq, Lk, H, dtype, scale=0.125, what=""):
-    """Asserts bound 1 on every element of the attention output; returns the worst error / bound."""
-    o64, pv, vmax = attn64(q, k, v, num_seq, Lq, Lk, H, scale)
-    bound = ulp16(o64, dtype) + U_P[dtype] * pv + 2.0 ** -20 * vmax
-    o = out.double()
-    assert torch.isfinite(o).all(), f"{what}: non-finite outputs"
-    ratio = ((o - o64).abs() / bound)
-    worst = ratio.max().item()
-    i = int(ratio.view(-1).argmax())
-    assert worst <= 1.0, (f"{what}: {int((ratio > 1).sum())} of {o.numel()} elements beyond bound 1; worst "
-                          f"{worst:.3g} x bound at {divmod(i, o.shape[1])}: out {o.view(-1)[i].item()!r} "
-                          f"ref {o64.view(-1)[i].item()!r}")
+def check_attn_bound1(out, q, k, v, num_seq, Lq, Lk, H, dtype, scale=0.125, what="", budget=1 << 25):
+    """Asserts bound 1 on every element of the attention output; returns the worst error / bound.  The float64 softmax
+    is built per sequence, head and block of queries, at most `budget` probabilities at a time (the global attention's
+    whole P would not fit in memory).  max|V| is taken over the sequence and head."""
+    qb = max(1, min(Lq, budget // max(Lk, 1)))
+    worst, n_bad, at = 0.0, 0, None
+    for s in range(num_seq):
+        for h in range(H):
+            cols = slice(64 * h, 64 * h + 64)
+            ks, vs = k[s * Lk:(s + 1) * Lk, cols], v[s * Lk:(s + 1) * Lk, cols]
+            vmax = vs.double().abs().max()
+            for r0 in range(0, Lq, qb):
+                rows = slice(s * Lq + r0, s * Lq + min(Lq, r0 + qb))
+                o64, pv = attn64(q[rows, cols], ks, vs, Lk, scale)
+                bound = ulp16(o64, dtype) + U_P[dtype] * pv + 2.0 ** -20 * vmax
+                o = out[rows, cols].double()
+                assert torch.isfinite(o).all(), f"{what}: non-finite outputs"
+                ratio = (o - o64).abs() / bound
+                n_bad += int((ratio > 1).sum())
+                w = ratio.max().item()
+                if w > worst:
+                    i = int(ratio.view(-1).argmax())
+                    worst, at = w, (rows.start + i // 64, 64 * h + i % 64, o.view(-1)[i].item(), o64.view(-1)[i].item())
+    assert worst <= 1.0, (f"{what}: {n_bad} of {out.shape[0] * H * 64} elements beyond bound 1; worst {worst:.3g} x "
+                          f"bound at ({at[0]}, {at[1]}): out {at[2]!r} ref {at[3]!r}")
     return worst
