@@ -109,6 +109,9 @@ SIGNATURES = {
                                c_int64, c_int, c_void_p, c_void_p, c_int64, c_void_p, c_void_p, c_void_p],
     "iggt_pointcloud_compact": [c_void_p, c_void_p, c_void_p, c_int64, c_void_p, c_void_p, c_void_p, c_void_p,
                                 c_void_p],
+    "iggt_mask_overlaps": [c_void_p, c_int64, c_int64, c_void_p, c_int64, c_int64, c_int64, c_void_p, c_void_p,
+                           c_void_p, c_void_p],
+    "iggt_linear_sum_assignment": [c_void_p, c_int64, c_int64, c_void_p, c_void_p],
     "iggt_avgpool2_nhwc": [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p],
     "iggt_sample_bilinear_nhwc": [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p],
     "iggt_corr_sample": [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int,

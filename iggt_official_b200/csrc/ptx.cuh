@@ -224,6 +224,35 @@ __device__ __forceinline__ void wgmma_m64n64k16_rs_tb(float (&d)[32], const uint
   else IGGT_WGMMA_RS_TB_64("f16");
 }
 
+// 8-bit integer form: D (+)= A[smem desc] * B[smem desc] with unsigned bytes, s32 accumulators (exact integer sums);
+// both operands K-major (8-bit wgmma has no transposed form), k32 per instruction = 32 bytes of the 128-byte swizzle row,
+// so the descriptors step exactly as for the 16-bit k16 forms.  Same fragment layout as above, s32 elements.
+template <int R>
+__device__ __forceinline__ void reg_fence(uint32_t (&d)[R]) {
+#pragma unroll
+  for (int i = 0; i < R; ++i) asm volatile("" : "+r"(d[i])::"memory");
+}
+#define IGGT_R8(o) "+r"(d[o]), "+r"(d[o + 1]), "+r"(d[o + 2]), "+r"(d[o + 3]), "+r"(d[o + 4]), "+r"(d[o + 5]), \
+                   "+r"(d[o + 6]), "+r"(d[o + 7])
+__device__ __forceinline__ void wgmma_m64n8k32_u8(uint32_t (&d)[4], uint64_t a_desc, uint64_t b_desc) {
+  asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %6, 0;\n\t"
+               "wgmma.mma_async.sync.aligned.m64n8k32.s32.u8.u8 {%0, %1, %2, %3}, %4, %5, p;\n\t}\n"
+               : "+r"(d[0]), "+r"(d[1]), "+r"(d[2]), "+r"(d[3])
+               : "l"(a_desc), "l"(b_desc), "r"(1));
+}
+__device__ __forceinline__ void wgmma_m64n64k32_u8(uint32_t (&d)[32], uint64_t a_desc, uint64_t b_desc) {
+  asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
+               "wgmma.mma_async.sync.aligned.m64n64k32.s32.u8.u8 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p;\n\t}\n"
+               : IGGT_R8(0), IGGT_R8(8), IGGT_R8(16), IGGT_R8(24)
+               : "l"(a_desc), "l"(b_desc), "r"(1));
+}
+__device__ __forceinline__ void wgmma_m64n128k32_u8(uint32_t (&d)[64], uint64_t a_desc, uint64_t b_desc) {
+  asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
+               "wgmma.mma_async.sync.aligned.m64n128k32.s32.u8.u8 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p;\n\t}\n"
+               : IGGT_R8(0), IGGT_R8(8), IGGT_R8(16), IGGT_R8(24), IGGT_R8(32), IGGT_R8(40), IGGT_R8(48), IGGT_R8(56)
+               : "l"(a_desc), "l"(b_desc), "r"(1));
+}
+
 // ---------------------------------------------------------------- descriptors
 // wgmma shared-memory matrix descriptor (sm_90): start>>4 [0,14), LBO>>4 [16,30), SBO>>4 [32,46), layout type [62,64)
 // (1 = SWIZZLE_128B).  128-byte swizzle: rows of 128 B (64 x 16-bit), 8-row atoms 1024 B apart (SBO); for a K-major

@@ -28,7 +28,7 @@ inline EncodeTiledFn get_encode_fn() {
   return fn;
 }
 
-enum TmDtype { TM_F16 = 0, TM_BF16 = 1, TM_F32 = 2 };
+enum TmDtype { TM_F16 = 0, TM_BF16 = 1, TM_F32 = 2, TM_U8 = 3 };
 
 // Generic rank<=4 tiled map. dims[0] is the contiguous dimension; strides_bytes[i] is the pitch of
 // dimension i+1 (rank-1 entries). 128-byte swizzle; out-of-bounds elements read as zero.
@@ -38,6 +38,7 @@ inline int make_tmap(CUtensorMap* out, TmDtype dt, int rank, const void* base, c
   if (!fn) return -1;
   CUtensorMapDataType cdt = dt == TM_F16    ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16
                             : dt == TM_BF16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16
+                            : dt == TM_U8   ? CU_TENSOR_MAP_DATA_TYPE_UINT8
                                             : CU_TENSOR_MAP_DATA_TYPE_FLOAT32;
   cuuint64_t gdim[5];
   cuuint64_t gstr[5];
@@ -65,7 +66,7 @@ inline int make_tmap(CUtensorMap* out, TmDtype dt, int rank, const void* base, c
 // Row-major [rows, cols] matrix with row pitch ld (elements); box = {box_cols, box_rows}.
 inline int make_tmap_2d(CUtensorMap* out, TmDtype dt, const void* base, uint64_t rows, uint64_t cols,
                         uint64_t ld, uint32_t box_cols, uint32_t box_rows) {
-  uint64_t es = (dt == TM_F32) ? 4 : 2;
+  uint64_t es = dt == TM_F32 ? 4 : dt == TM_U8 ? 1 : 2;
   uint64_t dims[2] = {cols, rows};
   uint64_t str[1] = {ld * es};
   uint32_t box[2] = {box_cols, box_rows};

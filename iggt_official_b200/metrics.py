@@ -12,7 +12,12 @@ Inputs are the reference's ndarrays or CUDA tensors (used in place) in its shape
 (N,3,4) or (N,4,4).  Depth is evaluated in float32.  Two differences remain: the sums are fp64 where the reference
 sums float32 terms pairwise in float32, and the resize follows scipy.ndimage.zoom(order=0, grid_mode=True), which is
 what skimage.transform.resize(order=0) calls.  4x4 poses are widened to fp64 like 3x4 ones (the reference keeps a
-float32 4x4 in float32).  No import of skimage, pandas, tqdm, scipy or cv2."""
+float32 4x4 in float32).  No import of skimage, pandas, tqdm, scipy or cv2.
+
+Instance masks (iggt/metrics.py:16-80): calculate_iou and evaluate_matched_instances with the reference's results and
+result types.  The device does all the pixel-sized work in one launch (csrc/instances.cu: exact intersection counts and
+mask sizes on the 8-bit tensor cores); the K x P rest (IoU, 1 - IoU, the assignment, the threshold and the means) is
+formed on the host in numpy with the reference's dtypes, the assignment by scipy's algorithm restated in the library."""
 import json
 import logging
 from typing import Any, Dict, Optional, Tuple
@@ -88,6 +93,122 @@ def _frame_metrics(r, total, alignment):
     m["total_pixels"] = total
     m["valid_ratio"] = np.int64(valid) / total
     return m
+
+
+def _is_cuda(x):
+    return isinstance(x, torch.Tensor) and x.is_cuda
+
+
+def _is_bool(m):
+    return m.dtype == torch.bool if isinstance(m, torch.Tensor) else m.dtype == np.bool_
+
+
+def _mask_rows(masks, name):
+    """masks: a stacked [K, ...] bool ndarray / tensor or a sequence of bool masks -> (list of per-mask arrays or the
+    stack itself, K, mask shape).  Non-bool dtypes raise TypeError, masks of different shapes ValueError."""
+    if isinstance(masks, (np.ndarray, torch.Tensor)):
+        if not _is_bool(masks):
+            raise TypeError(f"{name}: expected boolean masks, got {masks.dtype}")
+        if masks.ndim < 1:
+            raise ValueError(f"{name}: expected a stack [K, ...] of masks, got a scalar")
+        return masks, masks.shape[0], tuple(masks.shape[1:])
+    rows = [m if isinstance(m, (np.ndarray, torch.Tensor)) else np.asarray(m) for m in masks]
+    shape = None
+    for m in rows:
+        if not _is_bool(m):
+            raise TypeError(f"{name}: expected boolean masks, got {m.dtype}")
+        if shape is None:
+            shape = tuple(m.shape)
+        elif tuple(m.shape) != shape:
+            raise ValueError(f"{name}: masks of different shapes {shape} and {tuple(m.shape)}")
+    return rows, len(rows), shape
+
+
+def _mask_stack(masks, K, n, device):
+    """-> uint8 CUDA [K, ld] 0/1 stack for iggt_mask_overlaps.  A contiguous CUDA bool stack whose rows are a multiple
+    of 16 bytes is used in place; anything else is copied once into a zero-padded [K, round_up(n, 16)] buffer."""
+    if isinstance(masks, torch.Tensor) and masks.is_cuda and masks.device == device and masks.is_contiguous() \
+            and n % 16 == 0 and masks.data_ptr() % 16 == 0:
+        return masks.view(K, n).view(torch.uint8)
+    ld = (n + 15) // 16 * 16
+    if isinstance(masks, torch.Tensor):
+        buf = torch.zeros((K, ld), dtype=torch.uint8, device=device)
+        buf[:, :n].copy_(masks.reshape(K, n).to(device=device))
+        return buf
+    if isinstance(masks, np.ndarray) or not any(_is_cuda(m) for m in masks):
+        host = np.zeros((K, ld), dtype=np.uint8)
+        if isinstance(masks, np.ndarray):
+            host[:, :n] = masks.reshape(K, n)
+        else:
+            for i, m in enumerate(masks):
+                host[i, :n] = m.reshape(-1).numpy() if isinstance(m, torch.Tensor) else np.asarray(m).reshape(-1)
+        return torch.from_numpy(host).to(device)
+    buf = torch.zeros((K, ld), dtype=torch.uint8, device=device)
+    for i, m in enumerate(masks):
+        src = m.reshape(-1) if isinstance(m, torch.Tensor) else torch.from_numpy(np.ascontiguousarray(m).reshape(-1))
+        buf[i, :n].copy_(src.to(device=device))
+    return buf
+
+
+def _mask_counts(gt_masks, pred_masks):
+    """(inter [K,P], gsize [K], psize [P]) int64 ndarrays of two non-empty mask sets, from one device launch and one
+    copy to the host."""
+    g, K, gshape = _mask_rows(gt_masks, "gt_masks")
+    p, P, pshape = _mask_rows(pred_masks, "pred_masks")
+    if gshape != pshape:
+        raise ValueError(f"gt masks {gshape} and predicted masks {pshape} differ in shape")
+    n = int(np.prod(gshape, dtype=np.int64))
+    def tensors(m):
+        return [m] if isinstance(m, torch.Tensor) else [] if isinstance(m, np.ndarray) else m
+    device = _device_of(*tensors(g), *tensors(p))
+    if n == 0:
+        z = np.zeros
+        return z((K, P), np.int64), z(K, np.int64), z(P, np.int64)
+    counts = ops.mask_overlaps(_mask_stack(g, K, n, device), _mask_stack(p, P, n, device), n).cpu().numpy()
+    return counts[:K * P].reshape(K, P), counts[K * P:K * P + K], counts[K * P + K:]
+
+
+def _matched_from_counts(inter, gsize, psize, iou_threshold=0.5):
+    """evaluate_matched_instances' results from the exact counts (inter [K,P], gsize [K], psize [P] int64, K, P > 0),
+    with the reference's dtypes: an fp64 IoU matrix of int64 / int64 quotients (0.0 where the union is empty), the
+    assignment of 1 - IoU, then the threshold and the numpy means of the matched pairs."""
+    inter = np.asarray(inter, np.int64)
+    gsize, psize = np.asarray(gsize, np.int64), np.asarray(psize, np.int64)
+    union = gsize[:, None] + psize[None, :] - inter
+    iou_matrix = np.zeros(inter.shape)
+    pos = union > 0
+    iou_matrix[pos] = inter[pos] / union[pos]
+    gt_indices, pred_indices = ops.linear_sum_assignment(1 - iou_matrix)
+    matches, matched_ious, matched_accs = [], [], []
+    for gt_idx, pred_idx in zip(gt_indices, pred_indices):
+        if iou_matrix[gt_idx, pred_idx] >= iou_threshold:
+            matches.append((gt_idx, pred_idx))
+            matched_ious.append(iou_matrix[gt_idx, pred_idx])
+            tp_pixels, gt_pixels = inter[gt_idx, pred_idx], gsize[gt_idx]
+            matched_accs.append(tp_pixels / gt_pixels if gt_pixels > 0 else 0)
+    if not matches:
+        return {"matched_miou": 0, "matched_macc": 0, "num_matches": 0}, []
+    return {"matched_miou": np.mean(matched_ious), "matched_macc": np.mean(matched_accs),
+            "num_matches": len(matches)}, matches
+
+
+def calculate_iou(mask1, mask2):
+    """IoU of two boolean masks of one shape (ndarrays or tensors): np.float64, or 0.0 when both are empty."""
+    mask1, mask2 = (m if isinstance(m, (np.ndarray, torch.Tensor)) else np.asarray(m) for m in (mask1, mask2))
+    inter, gsize, psize = _mask_counts(mask1[None], mask2[None])
+    intersection = inter[0, 0]
+    union = gsize[0] + psize[0] - intersection
+    return intersection / union if union > 0 else 0.0
+
+
+def evaluate_matched_instances(gt_masks, pred_masks, iou_threshold=0.5):
+    """Optimal one-to-one matching of gt and predicted instance masks by IoU (scipy's linear_sum_assignment on
+    1 - IoU), then the mean IoU and mean pixel accuracy (|g & p| / |g|) of the pairs with IoU >= iou_threshold.
+    Masks: a stacked [K, ...] bool ndarray / tensor or a sequence of bool masks, all of one shape.
+    Returns ({"matched_miou", "matched_macc", "num_matches"}, [(gt_index, pred_index), ...])."""
+    if len(gt_masks) == 0 or len(pred_masks) == 0:
+        return {"matched_miou": 0, "matched_macc": 0, "num_matches": 0}, []
+    return _matched_from_counts(*_mask_counts(gt_masks, pred_masks), iou_threshold)
 
 
 class DepthEvaluator:

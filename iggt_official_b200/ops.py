@@ -826,6 +826,36 @@ def depth_to_cam(depth, intr):
 
 
 # ---------------------------------------------------------------------------------------------------
+# Instance-mask evaluation (csrc/instances.cu)
+def mask_overlaps(g, p, n):
+    """g [K,ldg], p [P,ldp] uint8 0/1 CUDA stacks (unit column stride, 16-byte aligned rows, ldg, ldp multiples of 16),
+    the first n bytes of each row the mask -> counts [K*P + K + P] int64 on the device: the intersection counts [K,P]
+    row-major, then the gt row sizes [K], then the pred row sizes [P] (one buffer: one copy to the host)."""
+    assert g.is_cuda and p.device == g.device and g.dtype == p.dtype == torch.uint8
+    assert g.dim() == p.dim() == 2 and g.stride(1) == p.stride(1) == 1
+    K, P = g.shape[0], p.shape[0]
+    counts = torch.empty(K * P + K + P, dtype=torch.int64, device=g.device)
+    _call(g, "iggt_mask_overlaps", 2.0 * K * P * n, float(K + P) * n, g.data_ptr(), K, g.stride(0), p.data_ptr(), P,
+          p.stride(0), int(n), counts.data_ptr(), counts.data_ptr() + 8 * K * P, counts.data_ptr() + 8 * (K * P + K),
+          _STREAM)
+    return counts
+
+
+def linear_sum_assignment(cost):
+    """Host (no GPU): cost [nr,nc] float64 -> (rows, cols) int64, the pairs scipy.optimize.linear_sum_assignment(cost)
+    returns, in its order.  A non-finite cost raises RuntimeError."""
+    import numpy as np
+    cost = np.ascontiguousarray(cost, dtype=np.float64)
+    assert cost.ndim == 2
+    nr, nc = cost.shape
+    m = min(nr, nc)
+    rows, cols = np.empty(m, np.int64), np.empty(m, np.int64)
+    _lib.check(_lib.load().iggt_linear_sum_assignment(cost.ctypes.data, nr, nc, rows.ctypes.data, cols.ctypes.data),
+               "iggt_linear_sum_assignment")
+    return rows, cols
+
+
+# ---------------------------------------------------------------------------------------------------
 # Point-cloud export (csrc/pointcloud.cu; the selection in csrc/pca.cu)
 PC_COLOR_F32, PC_COLOR_U8 = 0, 1
 PC_MASK_BLACK, PC_MASK_WHITE = 1, 2

@@ -480,6 +480,23 @@ int iggt_depth_zero_outside(float* depth, int64_t S, int64_t n, const float* thr
  * promotes the pixel grid and the intrinsics to float64).  intr [S, 3, 3] fp64. */
 int iggt_depth_to_cam(const float* depth, const double* intr, int S, int H, int W, float* cam, iggt_stream_t stream);
 
+/* ---- Instance-mask evaluation (iggt/metrics.py:16-80 calculate_iou / evaluate_matched_instances; csrc/instances.cu). */
+
+/* Exact overlap counts of 0/1 byte masks: inter [K, P] int64 = number of pixels set in both g[i] and p[j], gsize [K]
+ * and psize [P] int64 = pixels set in each row, for g [K, n] (row pitch ldg bytes) and p [P, n] (row pitch ldp), in one
+ * read of the stacks (8-bit tensor-core GEMM G P^T with s32 partials per CTA, int64 totals by integer atomics: exact and
+ * bit-identical on repeated calls).  Mask bytes must be 0 or 1.  -1: K, P or n out of range (n < 2^31 - 128);
+ * -2: ldg / ldp below n or not multiples of 16, or g / p not 16-byte aligned (TMA row pitches). */
+int iggt_mask_overlaps(const uint8_t* g, int64_t K, int64_t ldg, const uint8_t* p, int64_t P, int64_t ldp, int64_t n,
+                       int64_t* inter, int64_t* gsize, int64_t* psize, iggt_stream_t stream);
+
+/* HOST function (no GPU): the optimal assignment of cost [nr, nc] (row-major fp64) as scipy 1.18's
+ * linear_sum_assignment(cost) returns it, pair for pair and in the same order: min(nr, nc) pairs (rows[k], cols[k]),
+ * rows ascending.  Crouse's shortest augmenting path for rectangular matrices, on the transpose when nr > nc, with
+ * scipy's column scan order and tie rule (among equal path costs an unassigned column is preferred).  -2: a non-finite
+ * cost. */
+int iggt_linear_sum_assignment(const double* cost, int64_t nr, int64_t nc, int64_t* rows, int64_t* cols);
+
 /* ---- Point-cloud export (visual_util.py:38-238 predictions_to_glb, called three times per scene by demo.py:642;
  * csrc/pointcloud.cu).  Points are fp32 [n, 3], 0 < n < 2^32, in pixel order. */
 
