@@ -7,8 +7,9 @@
 // For every kv tile and half, a consumer computes S = Q K^T (wgmma, both operands from 128B-swizzled shared memory,
 // fp32 in registers), runs the online softmax on the register fragment (row max / sum across the 4 threads of a row),
 // packs P to 16 bit straight into the A-operand registers of O += P V (wgmma with A from registers, V read MN-major
-// from shared memory) and keeps O in registers.  The two consumers interleave their softmax phases with each other's
-// MMAs.
+// from shared memory) and keeps O in registers.  Inside a consumer, the softmax of one 64 x 64 slice runs while the
+// P V of the slice before it is in flight (attn3_tile), and the two consumers run free, interleaving their softmax
+// phases with each other's MMAs.  Registers: setmaxnreg gives the producer warpgroup 40, the consumers 232.
 // Item schedule: Attn3Items below.
 #include <stdlib.h>
 #include "ptx.cuh"
@@ -111,6 +112,154 @@ struct Attn3Items {
   }
 };
 
+// Register state of a consumer warpgroup for one work item.  A slice is 64 query rows (half hh of the query tile)
+// x 64 keys (half kh of the kv tile).
+struct Attn3Frag {
+  float o[2][32];
+  float m[2][2], l[2][2];            // [half][row r / r + 8]: running max (raw score units), partial sum
+  float s[32];                       // S of the next slice, then its unpacked P
+  uint32_t pa[4][4];                 // P of the current slice as the A fragments of the 4 k16 steps of P V
+  float fac[2];                      // the current slice's rescale factors of O (rows r / r + 8)
+};
+
+struct Attn3Bars {
+  uint64_t *k_full, *k_empty, *v_full, *v_empty, *q_empty;
+};
+
+// S = Q K^T of one slice: rows [64 hh, +64) of the query tile at q_addr, keys [64 kh, +64) of the kv tile at k_addr
+template <bool BF16>
+__device__ __forceinline__ void attn3_issue_s(float (&d)[32], uint32_t q_addr, int hh, uint32_t k_addr, int kh) {
+  wgmma_fence();
+#pragma unroll
+  for (int kk = 0; kk < A3_D / 16; ++kk)
+    wgmma_m64n64k16_ss<BF16>(d, make_desc_sw128(q_addr + hh * (64 * 128) + kk * 32, 1024),
+                             make_desc_sw128(k_addr + kh * (64 * 128) + kk * 32, 1024), kk != 0 ? 1u : 0u);
+  wgmma_commit();
+}
+
+// Online softmax of a completed S fragment (each row is spread over the 4 threads of a quad): masks the keys past
+// kvalid, updates the running max m and sum l of its half, leaves the rescale factors of O in fac (first: the half's
+// first slice, which rescales nothing) and the unpacked P in s.
+__device__ __forceinline__ void attn3_softmax(float (&s)[32], float (&m)[2], float (&l)[2], float (&fac)[2], int kvalid,
+                                              bool first, float c, int quad) {
+  if (kvalid < 64) {                                   // only the ragged last kv tile
+#pragma unroll
+    for (int jj = 0; jj < 8; ++jj) {
+      const int col = 8 * jj + 2 * quad;
+      if (col >= kvalid) { s[4 * jj] = -INFINITY; s[4 * jj + 2] = -INFINITY; }
+      if (col + 1 >= kvalid) { s[4 * jj + 1] = -INFINITY; s[4 * jj + 3] = -INFINITY; }
+    }
+  }
+  float mx0 = s[0], mx1 = s[2];
+#pragma unroll
+  for (int jj = 0; jj < 8; ++jj) {
+    mx0 = fmaxf(mx0, fmaxf(s[4 * jj], s[4 * jj + 1]));
+    mx1 = fmaxf(mx1, fmaxf(s[4 * jj + 2], s[4 * jj + 3]));
+  }
+  mx0 = fmaxf(mx0, __shfl_xor_sync(0xffffffffu, mx0, 1));
+  mx0 = fmaxf(mx0, __shfl_xor_sync(0xffffffffu, mx0, 2));
+  mx1 = fmaxf(mx1, __shfl_xor_sync(0xffffffffu, mx1, 1));
+  mx1 = fmaxf(mx1, __shfl_xor_sync(0xffffffffu, mx1, 2));
+  const float mn0 = fmaxf(m[0], mx0), mn1 = fmaxf(m[1], mx1);
+  if (!first) {
+    // a fully masked slice leaves the running max in place (mn == m): f = 1
+    fac[0] = ex2_approx((m[0] - mn0) * c);
+    fac[1] = ex2_approx((m[1] - mn1) * c);
+    // its own rounding: contracted with the sum below into one fma, l (and so the output) would change in the last bit
+    l[0] = __fmul_rn(l[0], fac[0]);
+    l[1] = __fmul_rn(l[1], fac[1]);
+  }
+  m[0] = mn0; m[1] = mn1;
+  const float nmc0 = -mn0 * c, nmc1 = -mn1 * c;
+#pragma unroll
+  for (int kk = 0; kk < 4; ++kk) {
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int jj = 2 * kk + h;
+      s[4 * jj] = ex2_approx(fmaf(s[4 * jj], c, nmc0));
+      s[4 * jj + 1] = ex2_approx(fmaf(s[4 * jj + 1], c, nmc0));
+      s[4 * jj + 2] = ex2_approx(fmaf(s[4 * jj + 2], c, nmc1));
+      s[4 * jj + 3] = ex2_approx(fmaf(s[4 * jj + 3], c, nmc1));
+    }
+    const float* e = s + 8 * kk;
+    l[0] += (e[0] + e[1]) + (e[4] + e[5]);
+    l[1] += (e[2] + e[3]) + (e[6] + e[7]);
+  }
+}
+
+// P to 16 bit, as the A fragments of the 4 k16 steps of P V
+template <bool BF16>
+__device__ __forceinline__ void attn3_pack_p(uint32_t (&pa)[4][4], const float (&s)[32]) {
+#pragma unroll
+  for (int kk = 0; kk < 4; ++kk) {
+    const float* e = s + 8 * kk;
+    pa[kk][0] = pack16x2<BF16>(e[0], e[1]);      // row r,     keys 16 kk + 2 quad + {0, 1}
+    pa[kk][1] = pack16x2<BF16>(e[2], e[3]);      // row r + 8
+    pa[kk][2] = pack16x2<BF16>(e[4], e[5]);      // row r,     keys 16 kk + 8 + 2 quad + {0, 1}
+    pa[kk][3] = pack16x2<BF16>(e[6], e[7]);      // row r + 8
+  }
+}
+
+// One kv tile j of a consumer's item.  Its slices run (kh, hh) = (0,0), (0,1), (1,0), (1,1): each half still sees its
+// keys in order, and consecutive slices use different O halves.  On entry the P of the tile's first slice is packed
+// in f.pa; per slice n the consumer issues S_{n+1}, rescales its O half and issues PV_n, waits for S_{n+1} only, runs
+// the softmax of slice n + 1 while PV_n is in flight, then waits for PV_n and packs P_{n+1}.  No wgmma is in flight
+// between slices, so P needs one register buffer.  In the item's first kv tile the halves' first slices rescale
+// nothing; LAST (the item's last kv tile, whose last slice has no S_{n+1}) is compile-time, so that no wgmma is issued
+// under a runtime condition.
+template <bool BF16, bool LAST>
+__device__ __forceinline__ void attn3_tile(Attn3Frag& f, int j, bool first, int& st, uint32_t& ph,
+                                           const Attn3Bars& b, const uint8_t* sK, const uint8_t* sV, uint32_t q_addr,
+                                           int Lk, float c, int quad, int gtid) {
+  const uint32_t k_addr = smem_u32(sK + st * A3_TILE);
+  const uint32_t v_addr = smem_u32(sV + st * A3_TILE);
+  int nst = st + 1; uint32_t nph = ph;                     // stage of kv tile j + 1
+  if (nst == A3_STAGES) { nst = 0; nph ^= 1; }
+#pragma unroll
+  for (int sl = 0; sl < 4; ++sl) {
+    const int kh = sl >> 1, hh = sl & 1;
+    const bool has_next = sl < 3 || !LAST;
+    const int nkh = sl < 3 ? (sl + 1) >> 1 : 0, nhh = hh ^ 1;
+    // ---- S of the next slice (after the tile's last slice: the next kv tile's first)
+    if (sl < 3) {
+      attn3_issue_s<BF16>(f.s, q_addr, nhh, k_addr, nkh);
+    } else if (!LAST) {
+      mbar_wait(&b.k_full[nst], nph);
+      attn3_issue_s<BF16>(f.s, q_addr, 0, smem_u32(sK + nst * A3_TILE), 0);
+    }
+    // ---- O += P V of this slice  (V rows [64 kh, +64) of the kv tile)
+    float (&o)[32] = f.o[hh];
+    if (!first || kh > 0) {
+#pragma unroll
+      for (int jj = 0; jj < 8; ++jj) {
+        o[4 * jj] *= f.fac[0]; o[4 * jj + 1] *= f.fac[0]; o[4 * jj + 2] *= f.fac[1]; o[4 * jj + 3] *= f.fac[1];
+      }
+    }
+    if (sl == 0) mbar_wait(&b.v_full[st], ph);
+    wgmma_fence();
+#pragma unroll
+    for (int kk = 0; kk < 4; ++kk)
+      wgmma_m64n64k16_rs_tb<BF16>(o, f.pa[kk], make_desc_sw128(v_addr + kh * (64 * 128) + kk * 2048, 1024), 1u);
+    wgmma_commit();
+    if (has_next) {
+      // ---- softmax of the next slice while P V runs
+      wgmma_wait<1>();
+      reg_fence(f.s);
+      if (sl == 2 && gtid == 0) {
+        mbar_arrive(&b.k_empty[st]);                     // all four S of this kv tile are complete
+        if (LAST) mbar_arrive(b.q_empty);                // last use of this item's Q
+      }
+      const int nj = sl < 3 ? j : j + 1;
+      attn3_softmax(f.s, f.m[nhh], f.l[nhh], f.fac, Lk - nj * A3_BK - nkh * 64, first && sl == 0, c, quad);
+    }
+    wgmma_wait<0>();
+    reg_fence(o);
+    if (sl == 3 && gtid == 0) mbar_arrive(&b.v_empty[st]);   // the last P V of this kv tile has retired
+    if (has_next) attn3_pack_p<BF16>(f.pa, f.s);
+  }
+  st = nst; ph = nph;
+}
+
 template <bool BF16>
 __global__ void __launch_bounds__(A3_THREADS, 1)
 attention3_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
@@ -150,6 +299,7 @@ attention3_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant
   griddep_launch();
 
   if (warp < 4) {
+    reg_dealloc<40>();
     if (warp == 0 && lane == 0) {
       // ------------------------------------------------------------------ TMA producer
       int st = 0; uint32_t ph = 0;
@@ -191,13 +341,13 @@ attention3_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant
     }
   } else {
     // -------------------------------------------------------------------- consumers (one warpgroup per query tile)
+    reg_alloc<232>();
     const int t = (warp - 4) >> 2;                 // query tile
     const int gtid = threadIdx.x & 127;
     const int ew = (warp - 4) & 3;                 // warp inside the warpgroup: fragment rows [16 ew, 16 ew + 16) of a half
     const int quad = lane & 3;
     const float c = p.scale_log2;
-    int kst = 0; uint32_t kph = 0;
-    int vst = 0; uint32_t vph = 0;
+    int st = 0; uint32_t ph = 0;                   // K / V ring stage and parity of the current kv tile
     uint32_t item_cnt = 0;                         // items in which THIS tile took part
     Attn3Items items(p, static_cast<int>(gridDim.x), static_cast<int>(blockIdx.x));
     int qp, head, seq;
@@ -209,12 +359,11 @@ attention3_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant
       if (!b_active && t == 1) {
         // tile B has no rows in this item: only keep the shared K/V ring turning
         for (int j = j0; j < j1; ++j) {
-          mbar_wait(&k_full[kst], kph);
-          if (gtid == 0) mbar_arrive(&k_empty[kst]);
-          if (++kst == A3_STAGES) { kst = 0; kph ^= 1; }
-          mbar_wait(&v_full[vst], vph);
-          if (gtid == 0) mbar_arrive(&v_empty[vst]);
-          if (++vst == A3_STAGES) { vst = 0; vph ^= 1; }
+          mbar_wait(&k_full[st], ph);
+          if (gtid == 0) mbar_arrive(&k_empty[st]);
+          mbar_wait(&v_full[st], ph);
+          if (gtid == 0) mbar_arrive(&v_empty[st]);
+          if (++st == A3_STAGES) { st = 0; ph ^= 1; }
         }
         continue;
       }
@@ -222,104 +371,28 @@ attention3_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant
       ++item_cnt;
       const uint32_t q_addr = smem_u32(sQ + (qbuf * 2 + t) * A3_TILE);
       mbar_wait(&q_full[qbuf * 2 + t], qbpar);
-      float o[2][32];
-      float m[2][2], l[2][2];                      // [half][row r / r + 8]: running max (raw score units), partial sum
+      Attn3Frag f;
 #pragma unroll
       for (int hh = 0; hh < 2; ++hh) {
 #pragma unroll
-        for (int i = 0; i < 32; ++i) o[hh][i] = 0.f;
-        m[hh][0] = m[hh][1] = -INFINITY;
-        l[hh][0] = l[hh][1] = 0.f;
+        for (int i = 0; i < 32; ++i) f.o[hh][i] = 0.f;
+        f.m[hh][0] = f.m[hh][1] = -INFINITY;
+        f.l[hh][0] = f.l[hh][1] = 0.f;
       }
-      for (int j = j0; j < j1; ++j) {
-        mbar_wait(&k_full[kst], kph);
-        const uint32_t k_addr = smem_u32(sK + kst * A3_TILE);
-        const uint32_t v_addr = smem_u32(sV + vst * A3_TILE);
-        const int valid = p.Lk - j * A3_BK;            // keys of this tile that exist
-#pragma unroll
-        for (int hh = 0; hh < 2; ++hh) {
-#pragma unroll 1
-          for (int kh = 0; kh < 2; ++kh) {
-            // ---- S = Q K^T  (64 query rows x 64 keys: rows [64 hh, +64) of the tile, keys [64 kh, +64) of the kv tile)
-            float s[32];
-            wgmma_fence();
-#pragma unroll
-            for (int kk = 0; kk < A3_D / 16; ++kk)
-              wgmma_m64n64k16_ss<BF16>(s, make_desc_sw128(q_addr + hh * (64 * 128) + kk * 32, 1024),
-                                       make_desc_sw128(k_addr + kh * (64 * 128) + kk * 32, 1024), kk != 0 ? 1u : 0u);
-            wgmma_commit();
-            wgmma_wait<0>();
-            reg_fence(s);
-            if (hh == 1 && kh == 1 && gtid == 0) {
-              mbar_arrive(&k_empty[kst]);
-              if (j == j1 - 1) mbar_arrive(&q_empty[qbuf * 2 + t]);     // last use of this item's Q
-            }
-            const int kvalid = valid - kh * 64;
-            if (kvalid < 64) {                             // only the ragged last kv tile
-#pragma unroll
-              for (int jj = 0; jj < 8; ++jj) {
-                const int col = 8 * jj + 2 * quad;
-                if (col >= kvalid) { s[4 * jj] = -INFINITY; s[4 * jj + 2] = -INFINITY; }
-                if (col + 1 >= kvalid) { s[4 * jj + 1] = -INFINITY; s[4 * jj + 3] = -INFINITY; }
-              }
-            }
-            // ---- online softmax (each row is spread over the 4 threads of a quad)
-            float mx0 = s[0], mx1 = s[2];
-#pragma unroll
-            for (int jj = 0; jj < 8; ++jj) {
-              mx0 = fmaxf(mx0, fmaxf(s[4 * jj], s[4 * jj + 1]));
-              mx1 = fmaxf(mx1, fmaxf(s[4 * jj + 2], s[4 * jj + 3]));
-            }
-            mx0 = fmaxf(mx0, __shfl_xor_sync(0xffffffffu, mx0, 1));
-            mx0 = fmaxf(mx0, __shfl_xor_sync(0xffffffffu, mx0, 2));
-            mx1 = fmaxf(mx1, __shfl_xor_sync(0xffffffffu, mx1, 1));
-            mx1 = fmaxf(mx1, __shfl_xor_sync(0xffffffffu, mx1, 2));
-            const float mn0 = fmaxf(m[hh][0], mx0), mn1 = fmaxf(m[hh][1], mx1);
-            if (j > j0 || kh > 0) {
-              // a fully masked slice leaves the running max in place (mn == m): f = 1
-              const float f0 = ex2_approx((m[hh][0] - mn0) * c), f1 = ex2_approx((m[hh][1] - mn1) * c);
-#pragma unroll
-              for (int jj = 0; jj < 8; ++jj) {
-                o[hh][4 * jj] *= f0; o[hh][4 * jj + 1] *= f0; o[hh][4 * jj + 2] *= f1; o[hh][4 * jj + 3] *= f1;
-              }
-              l[hh][0] *= f0; l[hh][1] *= f1;
-            }
-            m[hh][0] = mn0; m[hh][1] = mn1;
-            const float nmc0 = -mn0 * c, nmc1 = -mn1 * c;
-            uint32_t pa[4][4];                             // P as the A fragments of the 4 k16 steps of P V
-#pragma unroll
-            for (int kk = 0; kk < 4; ++kk) {
-              float e[8];
-#pragma unroll
-              for (int h = 0; h < 2; ++h) {
-                const int jj = 2 * kk + h;
-                e[4 * h + 0] = ex2_approx(fmaf(s[4 * jj], c, nmc0));
-                e[4 * h + 1] = ex2_approx(fmaf(s[4 * jj + 1], c, nmc0));
-                e[4 * h + 2] = ex2_approx(fmaf(s[4 * jj + 2], c, nmc1));
-                e[4 * h + 3] = ex2_approx(fmaf(s[4 * jj + 3], c, nmc1));
-              }
-              l[hh][0] += (e[0] + e[1]) + (e[4] + e[5]);
-              l[hh][1] += (e[2] + e[3]) + (e[6] + e[7]);
-              pa[kk][0] = pack16x2<BF16>(e[0], e[1]);      // row r,     keys 16 kk + 2 quad + {0, 1}
-              pa[kk][1] = pack16x2<BF16>(e[2], e[3]);      // row r + 8
-              pa[kk][2] = pack16x2<BF16>(e[4], e[5]);      // row r,     keys 16 kk + 8 + 2 quad + {0, 1}
-              pa[kk][3] = pack16x2<BF16>(e[6], e[7]);      // row r + 8
-            }
-            // ---- O += P V  (V rows [64 kh, +64) of the kv tile)
-            if (hh == 0 && kh == 0) mbar_wait(&v_full[vst], vph);
-            wgmma_fence();
-#pragma unroll
-            for (int kk = 0; kk < 4; ++kk)
-              wgmma_m64n64k16_rs_tb<BF16>(o[hh], pa[kk], make_desc_sw128(v_addr + kh * (64 * 128) + kk * 2048, 1024), 1u);
-            wgmma_commit();
-            wgmma_wait<0>();
-            reg_fence(o[hh]);
-          }
-        }
-        if (gtid == 0) mbar_arrive(&v_empty[vst]);
-        if (++kst == A3_STAGES) { kst = 0; kph ^= 1; }
-        if (++vst == A3_STAGES) { vst = 0; vph ^= 1; }
-      }
+      const Attn3Bars bars_t{k_full, k_empty, v_full, v_empty, &q_empty[qbuf * 2 + t]};
+      // the item's first slice: S, softmax and P before the pipelined kv tiles
+      mbar_wait(&k_full[st], ph);
+      attn3_issue_s<BF16>(f.s, q_addr, 0, smem_u32(sK + st * A3_TILE), 0);
+      wgmma_wait<0>();
+      reg_fence(f.s);
+      attn3_softmax(f.s, f.m[0], f.l[0], f.fac, p.Lk - j0 * A3_BK, true, c, quad);
+      attn3_pack_p<BF16>(f.pa, f.s);
+      for (int j = j0; j < j1 - 1; ++j)
+        attn3_tile<BF16, false>(f, j, j == j0, st, ph, bars_t, sK, sV, q_addr, p.Lk, c, quad, gtid);
+      attn3_tile<BF16, true>(f, j1 - 1, j1 - 1 == j0, st, ph, bars_t, sK, sV, q_addr, p.Lk, c, quad, gtid);
+      const float (&o)[2][32] = f.o;
+      const float (&m)[2][2] = f.m;
+      const float (&l)[2][2] = f.l;
       // ---- epilogue of the item
 #pragma unroll
       for (int hh = 0; hh < 2; ++hh) {
