@@ -45,8 +45,6 @@ SIGNATURES = {
                                     c_void_p, c_int, c_void_p],
     "iggt_deconv_shuffle": [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p],
     "iggt_im2col3x3_s2": [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p],
-    "iggt_dpt_tail": [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int,
-                      c_void_p],
     "iggt_dpt_tail_fused": [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int,
                             c_int, c_int, c_int, c_int, c_void_p],
     "iggt_skinny_gemm": [c_void_p, c_int64, c_void_p, c_int64, c_void_p, c_void_p, c_void_p, c_int64, c_void_p,

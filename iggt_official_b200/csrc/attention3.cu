@@ -11,7 +11,6 @@
 // P V of the slice before it is in flight (attn3_tile), and the two consumers run free, interleaving their softmax
 // phases with each other's MMAs.  Registers: setmaxnreg gives the producer warpgroup 40, the consumers 232.
 // Item schedule: Attn3Items below.
-#include <stdlib.h>
 #include "ptx.cuh"
 #include "tmap.cuh"
 #include "launch.cuh"
@@ -500,19 +499,14 @@ double attn3_cost(int num_seq, int Lq, int Lk, int H, int splits, int sms) {
   }
   return cost;
 }
-// kv splits that minimise attn3_cost (1 = no split); IGGT_ATTN_SPLITS forces a value
+// kv splits that minimise attn3_cost (1 = no split)
 int attn3_plan_splits(int num_seq, int Lq, int Lk, int H, int sms) {
-  static const int forced = [] { const char* e = getenv("IGGT_ATTN_SPLITS"); return e ? atoi(e) : 0; }();
   const int n_kv = (Lk + A3_BK - 1) / A3_BK;
   int best = 1;
-  if (forced > 0) {
-    best = forced < n_kv ? forced : n_kv;
-  } else {
-    double bc = attn3_cost(num_seq, Lq, Lk, H, 1, sms);
-    for (int s = 2; s <= 8 && s <= n_kv; ++s) {
-      const double c = attn3_cost(num_seq, Lq, Lk, H, s, sms);
-      if (c < 0.95 * bc) { bc = c; best = s; }        // a split must buy at least 5 %
-    }
+  double bc = attn3_cost(num_seq, Lq, Lk, H, 1, sms);
+  for (int s = 2; s <= 8 && s <= n_kv; ++s) {
+    const double c = attn3_cost(num_seq, Lq, Lk, H, s, sms);
+    if (c < 0.95 * bc) { bc = c; best = s; }          // a split must buy at least 5 %
   }
   const int tps = (n_kv + best - 1) / best;
   return (n_kv + tps - 1) / tps;                       // effective splits (no empty range)
@@ -526,8 +520,7 @@ void attn3_shape(Attn3Params& p, int num_seq, int Lq, int Lk, int H, int splits 
   p.tiles_per_split = (n_kv + p.kv_splits - 1) / p.kv_splits;
   p.ws_o = nullptr; p.ws_ml = nullptr;
   p.total_items = num_seq * H * p.q_pairs * p.kv_splits;
-  static const int lpt = [] { const char* e = getenv("IGGT_ATTN_LPT"); return e ? atoi(e) : 1; }();
-  p.light_tail = (lpt && (q_tiles & 1) && p.q_pairs > 1) ? 1 : 0;    // odd tile count: the last pair has no tile B
+  p.light_tail = ((q_tiles & 1) && p.q_pairs > 1) ? 1 : 0;    // odd tile count: the last pair has no tile B
 }
 }  // namespace
 

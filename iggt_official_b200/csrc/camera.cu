@@ -20,7 +20,6 @@
 // fp32 accumulation, 16-bit weights, activations to ~2^-22 (fp16 weights) / 2^-16 (bf16) relative - within rounding of the
 // arithmetic of iggt_skinny_gemm / iggt_small_attention, which this kernel replaces for M <= 16 (larger B*S keep the
 // per-layer launches).
-#include <stdlib.h>
 #include "ptx.cuh"
 #include "tmap.cuh"
 #include "launch.cuh"
@@ -64,15 +63,8 @@ struct CamProgram {
   CamPhase ph[CAM_MAX_PHASES];
   int n_phases, iters, M, Mpad, B, S;
   unsigned* barrier;           // zeroed before the launch
-  unsigned long long* dbg;     // optional (IGGT_CAMERA_DEBUG=1): CTA 0 stamps %globaltimer at 4 points of every phase
-  int dbg_mode;                // 2: consumers skip the arithmetic (pure weight-streaming rate; results are garbage)
 };
 
-__device__ __forceinline__ unsigned long long cam_now() {
-  unsigned long long t;
-  asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
-  return t;
-}
 __device__ __forceinline__ unsigned ld_acquire_u32(const unsigned* p) {
   unsigned v;
   asm volatile("ld.acquire.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
@@ -192,9 +184,6 @@ camera_head_kernel(const __grid_constant__ CamProgram prog) {
     for (int p = 0; p < prog.n_phases; ++p) {
       const CamPhase& P = prog.ph[p];
       if ((P.flags & CF_ONCE) && it > 0) continue;
-      unsigned long long* stamp = (prog.dbg && cta == 0 && tid == 0) ? prog.dbg + (it * CAM_MAX_PHASES + p) * 4 : nullptr;
-      long long wait_clk = 0;
-      if (stamp) stamp[0] = cam_now();
       if (P.type == PH_GEMM) {
         const int tiles = (P.N + CAM_COLS - 1) / CAM_COLS;
         const int nchunks = (P.K + KX - 1) / KX;                         // activation chunks of KX
@@ -272,7 +261,6 @@ camera_head_kernel(const __grid_constant__ CamProgram prog) {
                 }
               }
               named_bar_sync(2, 256);
-              if (stamp && ch == 0) stamp[1] = cam_now();
             }
 #pragma unroll
             for (int ti = 0; ti < 4; ++ti) {
@@ -280,34 +268,32 @@ camera_head_kernel(const __grid_constant__ CamProgram prog) {
             // ---- weight stages of this chunk (1024 k each)
             for (int ks = 0; ks < (kn + CAM_KS - 1) / CAM_KS; ++ks) {
               mbar_wait(&full[st], ph);
-              if (prog.dbg_mode != 2) {
-                const uint8_t* wst = sW + st * CAM_W_BYTES;
-                const int steps = min(CAM_KS, kn - ks * CAM_KS + 15) / 16;      // k steps of 16 in this stage (64, or 1 for K = 16)
-                for (int s16 = warp; s16 < steps; s16 += 8) {
-                  const int kk = ks * CAM_KS + s16 * 16;                  // chunk-local k of this step
-                  // A fragments: rows g (and g + 8 when more than 8 rows are staged), k = kk + 2 tq (+ 8)
-                  const uint32_t ah0 = *reinterpret_cast<const uint32_t*>(xs + g * KXP + kk + 2 * tq);
-                  const uint32_t ah2 = *reinterpret_cast<const uint32_t*>(xs + g * KXP + kk + 8 + 2 * tq);
-                  const uint32_t al0 = *reinterpret_cast<const uint32_t*>(xlo + g * KXP + kk + 2 * tq);
-                  const uint32_t al2 = *reinterpret_cast<const uint32_t*>(xlo + g * KXP + kk + 8 + 2 * tq);
-                  uint32_t ah1 = 0, ah3 = 0, al1 = 0, al3 = 0;
-                  if constexpr (MP == 16) {
-                    ah1 = *reinterpret_cast<const uint32_t*>(xs + (g + 8) * KXP + kk + 2 * tq);
-                    ah3 = *reinterpret_cast<const uint32_t*>(xs + (g + 8) * KXP + kk + 8 + 2 * tq);
-                    al1 = *reinterpret_cast<const uint32_t*>(xlo + (g + 8) * KXP + kk + 2 * tq);
-                    al3 = *reinterpret_cast<const uint32_t*>(xlo + (g + 8) * KXP + kk + 8 + 2 * tq);
-                  }
-                  // B fragments from the swizzled stage: k group (64 k) q64, 16-byte chunk (2 j) ^ (col & 7), + 4 tq bytes
-                  const int q64 = s16 >> 2, j = (s16 & 3) * 2;
+              const uint8_t* wst = sW + st * CAM_W_BYTES;
+              const int steps = min(CAM_KS, kn - ks * CAM_KS + 15) / 16;      // k steps of 16 in this stage (64, or 1 for K = 16)
+              for (int s16 = warp; s16 < steps; s16 += 8) {
+                const int kk = ks * CAM_KS + s16 * 16;                  // chunk-local k of this step
+                // A fragments: rows g (and g + 8 when more than 8 rows are staged), k = kk + 2 tq (+ 8)
+                const uint32_t ah0 = *reinterpret_cast<const uint32_t*>(xs + g * KXP + kk + 2 * tq);
+                const uint32_t ah2 = *reinterpret_cast<const uint32_t*>(xs + g * KXP + kk + 8 + 2 * tq);
+                const uint32_t al0 = *reinterpret_cast<const uint32_t*>(xlo + g * KXP + kk + 2 * tq);
+                const uint32_t al2 = *reinterpret_cast<const uint32_t*>(xlo + g * KXP + kk + 8 + 2 * tq);
+                uint32_t ah1 = 0, ah3 = 0, al1 = 0, al3 = 0;
+                if constexpr (MP == 16) {
+                  ah1 = *reinterpret_cast<const uint32_t*>(xs + (g + 8) * KXP + kk + 2 * tq);
+                  ah3 = *reinterpret_cast<const uint32_t*>(xs + (g + 8) * KXP + kk + 8 + 2 * tq);
+                  al1 = *reinterpret_cast<const uint32_t*>(xlo + (g + 8) * KXP + kk + 2 * tq);
+                  al3 = *reinterpret_cast<const uint32_t*>(xlo + (g + 8) * KXP + kk + 8 + 2 * tq);
+                }
+                // B fragments from the swizzled stage: k group (64 k) q64, 16-byte chunk (2 j) ^ (col & 7), + 4 tq bytes
+                const int q64 = s16 >> 2, j = (s16 & 3) * 2;
 #pragma unroll
-                  for (int c = 0; c < 2; ++c) {
-                    const int col = c * 8 + g;
-                    const uint8_t* wr = wst + q64 * (CAM_COLS * 128) + col * 128 + tq * 4;
-                    const uint32_t b0 = *reinterpret_cast<const uint32_t*>(wr + ((j ^ (col & 7)) << 4));
-                    const uint32_t b1 = *reinterpret_cast<const uint32_t*>(wr + (((j + 1) ^ (col & 7)) << 4));
-                    cam_mma<BF16>(acc[ti][c], ah0, ah1, ah2, ah3, b0, b1);
-                    cam_mma<BF16>(acc[ti][c], al0, al1, al2, al3, b0, b1);
-                  }
+                for (int c = 0; c < 2; ++c) {
+                  const int col = c * 8 + g;
+                  const uint8_t* wr = wst + q64 * (CAM_COLS * 128) + col * 128 + tq * 4;
+                  const uint32_t b0 = *reinterpret_cast<const uint32_t*>(wr + ((j ^ (col & 7)) << 4));
+                  const uint32_t b1 = *reinterpret_cast<const uint32_t*>(wr + (((j + 1) ^ (col & 7)) << 4));
+                  cam_mma<BF16>(acc[ti][c], ah0, ah1, ah2, ah3, b0, b1);
+                  cam_mma<BF16>(acc[ti][c], al0, al1, al2, al3, b0, b1);
                 }
               }
               __syncwarp();
@@ -425,9 +411,7 @@ camera_head_kernel(const __grid_constant__ CamProgram prog) {
           }
         }
       }
-      if (stamp) stamp[2] = cam_now();
       cam_grid_sync(prog.barrier, target);
-      if (stamp) stamp[3] = cam_now() | (static_cast<unsigned long long>(wait_clk >> 6) << 48);   // + cycles/64 spent waiting for weights
     }
 }
 
@@ -445,7 +429,7 @@ int64_t cam_ws_floats(int M) { return static_cast<int64_t>(M) * (5 * CAM_DIM + 2
 
 extern "C" int64_t iggt_camera_head_workspace(int M) {
   if (M <= 0) return -1;
-  return cam_ws_floats(M) * 4 + 256 + 8 * CAM_MAX_PHASES * 4 * 8;     // + debug stamps [8 iters][32 phases][4]
+  return cam_ws_floats(M) * 4 + 256;
 }
 
 extern "C" int iggt_camera_head(const iggt_camera_weights* w, const float* tokens, int64_t ld_tokens, float* out,
@@ -470,7 +454,6 @@ extern "C" int iggt_camera_head(const iggt_camera_weights* w, const float* token
   ws.hdn = p; p += M * 1024;
   ws.pred = p; p += M * 16;
   ws.barrier = reinterpret_cast<unsigned*>((reinterpret_cast<uintptr_t>(p) + 127) & ~static_cast<uintptr_t>(127));
-  static const int dbg_env = [] { const char* e = getenv("IGGT_CAMERA_DEBUG"); return e ? atoi(e) : 0; }();
   cudaError_t e = cudaMemsetAsync(ws.barrier, 0, 4, s);
   if (e != cudaSuccess) return (int)e;
   e = cudaMemsetAsync(ws.pred, 0, M * 16 * 4, s);       // columns 9..15 of `pred` are the zero padding of embed_pose's K
@@ -478,8 +461,6 @@ extern "C" int iggt_camera_head(const iggt_camera_weights* w, const float* token
 
   CamProgram prog{};
   prog.iters = iters; prog.M = M; prog.Mpad = M <= 8 ? 8 : 16; prog.B = B; prog.S = S; prog.barrier = ws.barrier;
-  prog.dbg = (dbg_env && iters <= 8) ? reinterpret_cast<unsigned long long*>(ws.barrier + 32) : nullptr;   // +128 B
-  prog.dbg_mode = dbg_env;
   const TmDtype dt = dtype ? TM_BF16 : TM_F16;
   int nmaps = 0;
   // weights [N, K] row-major seen as {64 k, N, K / 64} (128B-swizzled rows of 64 k): one box = 16 columns x 1024 k

@@ -40,7 +40,7 @@ struct GemmParams {
   int num_m_tiles, num_n_tiles, num_k_blocks;
   const float* bias;   // [N] or nullptr
   const float* gamma;  // [N] (EPI_RESID32) or nullptr (=1)
-  int act;             // 0 none, 1 exact GELU, 2 ReLU, 3 LeakyReLU(0.01), 5 exact GELU (one-MUFU erfc form)
+  int act;             // 0 none, 1 exact GELU, 2 ReLU, 3 LeakyReLU(0.01)
   // EPI_QKV
   int qk_norm;         // apply LayerNorm(64) (eps 1e-5, affine) + RoPE to the q and k column ranges
   int C;               // embedding width: q = cols [0,C), k = [C,2C), v = [2C,3C)
@@ -407,13 +407,6 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
 #pragma unroll
               for (int i = 0; i < 64; i += 2) {
                 const float2 g = gelu_fast2(make_float2(round16<BF16>(v[i]), round16<BF16>(v[i + 1])));
-                v[i] = g.x; v[i + 1] = g.y;
-              }
-            } else if (p.act == 5) {
-              // the same GELU through the one-MUFU erfc form (ptx.cuh gelu_erfc2)
-#pragma unroll
-              for (int i = 0; i < 64; i += 2) {
-                const float2 g = gelu_erfc2(make_float2(round16<BF16>(v[i]), round16<BF16>(v[i + 1])));
                 v[i] = g.x; v[i + 1] = g.y;
               }
             } else if (p.act) {

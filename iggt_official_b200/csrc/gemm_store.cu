@@ -1,5 +1,4 @@
 // C-ABI launchers: 16-bit and 32-bit store epilogues (see include/iggt_b200.h).
-#include <stdlib.h>
 #include "gemm_launch.cuh"
 #include "../../include/iggt_b200.h"
 
@@ -60,9 +59,7 @@ extern "C" int iggt_gemm_store16(const void* A, int64_t lda, const void* W, int6
                                  int act, const void* addend, int add_rows, int64_t add_ld,
                                  iggt_stream_t stream) {
   GemmParams p{};
-  // IGGT_GELU=2: the one-MUFU erfc form of the same exact-erf GELU (A/B switch; default = the two-MUFU form)
-  static const int gelu_v = [] { const char* e = getenv("IGGT_GELU"); return e ? atoi(e) : 1; }();
-  p.bias = bias; p.act = (act == 1 && gelu_v == 2) ? 5 : act;
+  p.bias = bias; p.act = act;
   p.addend = addend; p.add_rows = add_rows > 0 ? add_rows : 1; p.add_ld = (int)add_ld;
   if (addend && (add_ld % 8)) return -2;
   return gemm_common(EPI_STORE16, A, lda, W, ldw, out, ldo, M, N, K, dtype, p, (cudaStream_t)stream);

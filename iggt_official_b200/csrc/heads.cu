@@ -137,49 +137,6 @@ im2col_s2_kernel(const uint4* __restrict__ x, uint4* __restrict__ A, int NB, int
   }
 }
 
-// Per-pixel tail: 1x1 conv 32 -> OC (fp32 weights) + head activation (iggt/heads/dpt_head.py:264-265,
-// iggt/heads/head_act.py:61-125).  mode 0: xyz=exp, conf=1+exp (depth); 1: xyz=sign*expm1|.|, conf=1+exp
-// (points); 2: raw, channels-first [NB,OC,H,W] (part_feat, iggt/heads/part_head.py:240-243).
-template <bool BF16, int OC>
-__global__ void __launch_bounds__(256)
-dpt_tail_kernel(const uint16_t* __restrict__ x, const float* __restrict__ w, const float* __restrict__ b,
-                float* __restrict__ out_main, float* __restrict__ out_conf, int64_t npix, int64_t hw, int mode) {
-  __shared__ float sw[OC * 32 + OC];
-  for (int i = threadIdx.x; i < OC * 32 + OC; i += blockDim.x) sw[i] = i < OC * 32 ? w[i] : b[i - OC * 32];
-  __syncthreads();
-  for (int64_t pix = blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x; pix < npix;
-       pix += static_cast<int64_t>(gridDim.x) * blockDim.x) {
-    float f[32];
-#pragma unroll
-    for (int q = 0; q < 4; ++q) {
-      float t[8];
-      unpack8<BF16>(__ldg(reinterpret_cast<const uint4*>(x + pix * 32) + q), t);
-#pragma unroll
-      for (int k = 0; k < 8; ++k) f[q * 8 + k] = t[k];
-    }
-    float o[OC];
-#pragma unroll
-    for (int c = 0; c < OC; ++c) {
-      float s = sw[OC * 32 + c];
-#pragma unroll
-      for (int k = 0; k < 32; ++k) s = fmaf(f[k], sw[c * 32 + k], s);
-      o[c] = s;
-    }
-    if (mode == 2) {
-      const int64_t n = pix / hw, r = pix % hw;
-#pragma unroll
-      for (int c = 0; c < OC; ++c) out_main[(n * OC + c) * hw + r] = o[c];
-    } else {
-#pragma unroll
-      for (int c = 0; c < OC - 1; ++c) {
-        const float v = o[c];
-        out_main[pix * (OC - 1) + c] = mode == 0 ? expf(v) : copysignf(expm1f(fabsf(v)), v);
-      }
-      out_conf[pix] = 1.0f + expf(o[OC - 1]);
-    }
-  }
-}
-
 // out[m, n] = (resid ? resid[m,n] : 0) + gamma[n] * act(x[m,:] . W[n,:] + bias[n]),  M <= 8 rows per launch
 // (the host loops over row chunks), fp32 activations, 16-bit weights streamed once.  Camera-head Linear layers
 // (iggt/heads/camera_head.py:83-154): 8 rows against up to 33 MB of weights -> purely weight-bandwidth bound, so
@@ -365,19 +322,6 @@ extern "C" int iggt_im2col3x3_s2(const void* x, void* A, int NB, int h, int w, i
   const int ho = (h - 1) / 2 + 1, wo = (w - 1) / 2 + 1;
   const int64_t total = static_cast<int64_t>(NB) * ho * wo * 9 * (C / 8);
   im2col_s2_kernel<<<grid_for(total), 256, 0, (cudaStream_t)stream>>>((const uint4*)x, (uint4*)A, NB, h, w, C, ho, wo);
-  return (int)cudaGetLastError();
-}
-
-extern "C" int iggt_dpt_tail(const void* x, const float* w, const float* b, float* out_main, float* out_conf,
-                             int NB, int H, int W, int OC, int mode, int dtype, iggt_stream_t stream) {
-  if (NB <= 0 || (OC != 2 && OC != 4 && OC != 8)) return -1;
-  if (mode != 2 && !out_conf) return -1;
-  const int64_t hw = static_cast<int64_t>(H) * W, npix = hw * NB;
-  cudaStream_t s = (cudaStream_t)stream;
-#define TAIL(BF, O) dpt_tail_kernel<BF, O><<<grid_for(npix), 256, 0, s>>>((const uint16_t*)x, w, b, out_main, out_conf, npix, hw, mode)
-  if (dtype) { if (OC == 2) TAIL(true, 2); else if (OC == 4) TAIL(true, 4); else TAIL(true, 8); }
-  else { if (OC == 2) TAIL(false, 2); else if (OC == 4) TAIL(false, 4); else TAIL(false, 8); }
-#undef TAIL
   return (int)cudaGetLastError();
 }
 

@@ -1,9 +1,9 @@
 // Kernels of the part (instance-feature) path that are not GEMM-shaped enough for the wgmma main loop:
 // small-C LayerNorm on 16-bit NHWC rows, the k4/s2/p1 ConvTranspose gather, the two 8x8-window attentions
 // (OCAB with 12x12 overlapping keys + relative-position bias and the reference's scrambled query windows;
-// HAB plain window self-attention), and the CAB channel-attention (squeeze-excite) pieces.
+// HAB plain window self-attention; the tensor-core kernels are in winattn.cuh), and the CAB channel-attention
+// (squeeze-excite) pieces.
 // Reference: iggt/heads/adaptor.py:140-226, iggt/heads/part_head.py:148-243, iggt/heads/window_sa.py.
-#include <stdlib.h>
 #include "ptx.cuh"
 #include "launch.cuh"
 #include "winattn.cuh"
@@ -99,224 +99,6 @@ col2im_k4s2p1_kernel(const uint16_t* __restrict__ Y, const float* __restrict__ b
   }
 }
 
-// OCAB attention (iggt/heads/window_sa.py:271-319), one CTA per (image, window, head), 256 threads.
-//   q windows: the reference partitions the (b, c, h, w)-permuted Q with a (b, h, w, c) partition, so
-//     q_win[n, t, f] = Q[b, yb*8+yi, x, cb*8+ci] with L = (n*64+t)*256+f decoded little-endian with radices
-//     (x:w, yi:8, ci:8, yb:h/8, cb:32)                                               (SURVEY F5 / E-15)
-//   k/v windows: 12x12 pixels around window (wy,wx) (rows 8wy-2 .. 8wy+9), zeros outside the map
-//   scores = (q * d^-0.5) k^T + table[rpi[t, j]][head]; softmax; out written to pixel (8wy+ty, 8wx+tx).
-constexpr int OC_WS = 8, OC_OWS = 12, OC_NQ = 64, OC_NK = 144, OC_D = 64, OC_C = 256;
-
-template <bool BF16>
-__global__ void __launch_bounds__(256)
-ocab_attention_kernel(const uint16_t* __restrict__ Q, const uint16_t* __restrict__ K, const uint16_t* __restrict__ V,
-                      const float* __restrict__ table, const int* __restrict__ rpi, uint16_t* __restrict__ out,
-                      int h, int w) {
-  extern __shared__ float sm[];
-  float* sq = sm;                              // [64][65]
-  float* sk = sq + OC_NQ * 65;                 // [144][65]
-  float* sv = sk + OC_NK * 65;                 // [144][64]
-  float* ss = sv + OC_NK * 64;                 // [64][145]
-  const int nwx = w / OC_WS, nwy = h / OC_WS;
-  const int head = blockIdx.x % 4;
-  const int win = (blockIdx.x / 4) % (nwx * nwy);
-  const int b = blockIdx.x / (4 * nwx * nwy);
-  const int wy = win / nwx, wx = win % nwx;
-  const int tid = threadIdx.x;
-  const float scale = 0.125f;                  // 64^-0.5
-  // scrambled query gather
-  for (int i = tid; i < OC_NQ * OC_D; i += 256) {
-    const int t = i / OC_D, d = i % OC_D;
-    int64_t L = (static_cast<int64_t>(win) * 64 + t) * OC_C + head * OC_D + d;
-    const int x = static_cast<int>(L % w); L /= w;
-    const int yi = static_cast<int>(L % 8); L /= 8;
-    const int ci = static_cast<int>(L % 8); L /= 8;
-    const int yb = static_cast<int>(L % nwy); L /= nwy;
-    const int cb = static_cast<int>(L);
-    sq[t * 65 + d] = ld16<BF16>(Q + ((static_cast<int64_t>(b) * h + yb * 8 + yi) * w + x) * OC_C + cb * 8 + ci) * scale;
-  }
-  for (int i = tid; i < OC_NK * OC_D; i += 256) {
-    const int j = i / OC_D, d = i % OC_D;
-    const int yy = wy * OC_WS - 2 + j / OC_OWS, xx = wx * OC_WS - 2 + j % OC_OWS;
-    float kv = 0.f, vv = 0.f;
-    if (yy >= 0 && yy < h && xx >= 0 && xx < w) {
-      const int64_t off = ((static_cast<int64_t>(b) * h + yy) * w + xx) * OC_C + head * OC_D + d;
-      kv = ld16<BF16>(K + off);
-      vv = ld16<BF16>(V + off);
-    }
-    sk[j * 65 + d] = kv;
-    sv[j * 64 + d] = vv;
-  }
-  __syncthreads();
-  {  // scores: thread -> 4 queries x 9 keys
-    const int tq = tid / 16, tk = tid % 16;
-    float acc[4][9];
-#pragma unroll
-    for (int a = 0; a < 4; ++a)
-#pragma unroll
-      for (int c = 0; c < 9; ++c) acc[a][c] = 0.f;
-    for (int d = 0; d < OC_D; ++d) {
-      float qa[4], kb[9];
-#pragma unroll
-      for (int a = 0; a < 4; ++a) qa[a] = sq[(tq * 4 + a) * 65 + d];
-#pragma unroll
-      for (int c = 0; c < 9; ++c) kb[c] = sk[(tk * 9 + c) * 65 + d];
-#pragma unroll
-      for (int a = 0; a < 4; ++a)
-#pragma unroll
-        for (int c = 0; c < 9; ++c) acc[a][c] = fmaf(qa[a], kb[c], acc[a][c]);
-    }
-#pragma unroll
-    for (int a = 0; a < 4; ++a)
-#pragma unroll
-      for (int c = 0; c < 9; ++c) {
-        const int t = tq * 4 + a, j = tk * 9 + c;
-        ss[t * 145 + j] = acc[a][c] + __ldg(table + __ldg(rpi + t * OC_NK + j) * 4 + head);
-      }
-  }
-  __syncthreads();
-  {  // softmax per row: warp handles 8 rows
-    const int warp = tid >> 5, lane = tid & 31;
-    for (int r = warp * 8; r < warp * 8 + 8; ++r) {
-      float mx = -INFINITY;
-      for (int j = lane; j < OC_NK; j += 32) mx = fmaxf(mx, ss[r * 145 + j]);
-#pragma unroll
-      for (int o = 16; o > 0; o >>= 1) mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, o));
-      float sum = 0.f;
-      for (int j = lane; j < OC_NK; j += 32) { const float e = expf(ss[r * 145 + j] - mx); ss[r * 145 + j] = e; sum += e; }
-#pragma unroll
-      for (int o = 16; o > 0; o >>= 1) sum += __shfl_xor_sync(0xffffffffu, sum, o);
-      const float inv = 1.0f / sum;
-      for (int j = lane; j < OC_NK; j += 32) ss[r * 145 + j] *= inv;
-    }
-  }
-  __syncthreads();
-  {  // P V: thread -> 4 queries x 4 dims
-    const int tq = tid / 16, td = tid % 16;
-    float acc[4][4];
-#pragma unroll
-    for (int a = 0; a < 4; ++a)
-#pragma unroll
-      for (int c = 0; c < 4; ++c) acc[a][c] = 0.f;
-    for (int j = 0; j < OC_NK; ++j) {
-      float pa[4], vb[4];
-#pragma unroll
-      for (int a = 0; a < 4; ++a) pa[a] = ss[(tq * 4 + a) * 145 + j];
-#pragma unroll
-      for (int c = 0; c < 4; ++c) vb[c] = sv[j * 64 + td * 4 + c];
-#pragma unroll
-      for (int a = 0; a < 4; ++a)
-#pragma unroll
-        for (int c = 0; c < 4; ++c) acc[a][c] = fmaf(pa[a], vb[c], acc[a][c]);
-    }
-#pragma unroll
-    for (int a = 0; a < 4; ++a) {
-      const int t = tq * 4 + a;
-      const int yy = wy * OC_WS + t / OC_WS, xx = wx * OC_WS + t % OC_WS;
-      uint16_t* dst = out + ((static_cast<int64_t>(b) * h + yy) * w + xx) * OC_C + head * OC_D + td * 4;
-      uint2 u;
-      u.x = pack16x2<BF16>(acc[a][0], acc[a][1]);
-      u.y = pack16x2<BF16>(acc[a][2], acc[a][3]);
-      *reinterpret_cast<uint2*>(dst) = u;
-    }
-  }
-}
-constexpr int OCAB_SMEM = (OC_NQ * 65 + OC_NK * 65 + OC_NK * 64 + OC_NQ * 145) * 4;
-
-// HAB window self-attention (iggt/heads/window_sa.py:201-227 + iggt/heads/block.py:113-130): 8x8 windows,
-// 4 heads x 32, scale 32^-0.5, no bias / mask.  qkv [NB,h,w,384] = [q | k | v], head-major inside each.
-// One CTA per (image, window, head), 128 threads.
-template <bool BF16>
-__global__ void __launch_bounds__(128)
-window_attention_kernel(const uint16_t* __restrict__ qkv, uint16_t* __restrict__ out, int h, int w) {
-  __shared__ float sq[64 * 33], sk[64 * 33], sv[64 * 32], ss[64 * 65];
-  const int nwx = w / 8, nwy = h / 8;
-  const int head = blockIdx.x % 4;
-  const int win = (blockIdx.x / 4) % (nwx * nwy);
-  const int b = blockIdx.x / (4 * nwx * nwy);
-  const int wy = win / nwx, wx = win % nwx;
-  const int tid = threadIdx.x;
-  const float scale = 0.17677669529663687f;    // 32^-0.5
-  for (int i = tid; i < 64 * 32; i += 128) {
-    const int t = i / 32, d = i % 32;
-    const int64_t pix = (static_cast<int64_t>(b) * h + wy * 8 + t / 8) * w + wx * 8 + t % 8;
-    const uint16_t* p = qkv + pix * 384 + head * 32 + d;
-    sq[t * 33 + d] = ld16<BF16>(p) * scale;
-    sk[t * 33 + d] = ld16<BF16>(p + 128);
-    sv[t * 32 + d] = ld16<BF16>(p + 256);
-  }
-  __syncthreads();
-  {  // scores: thread -> 4 q x 8 k
-    const int tq = tid / 8, tk = tid % 8;
-    float acc[4][8];
-#pragma unroll
-    for (int a = 0; a < 4; ++a)
-#pragma unroll
-      for (int c = 0; c < 8; ++c) acc[a][c] = 0.f;
-    for (int d = 0; d < 32; ++d) {
-      float qa[4], kb[8];
-#pragma unroll
-      for (int a = 0; a < 4; ++a) qa[a] = sq[(tq * 4 + a) * 33 + d];
-#pragma unroll
-      for (int c = 0; c < 8; ++c) kb[c] = sk[(tk * 8 + c) * 33 + d];
-#pragma unroll
-      for (int a = 0; a < 4; ++a)
-#pragma unroll
-        for (int c = 0; c < 8; ++c) acc[a][c] = fmaf(qa[a], kb[c], acc[a][c]);
-    }
-#pragma unroll
-    for (int a = 0; a < 4; ++a)
-#pragma unroll
-      for (int c = 0; c < 8; ++c) ss[(tq * 4 + a) * 65 + tk * 8 + c] = acc[a][c];
-  }
-  __syncthreads();
-  {
-    const int warp = tid >> 5, lane = tid & 31;
-    for (int r = warp * 16; r < warp * 16 + 16; ++r) {
-      const float a0 = ss[r * 65 + lane], a1 = ss[r * 65 + lane + 32];
-      float mx = fmaxf(a0, a1);
-#pragma unroll
-      for (int o = 16; o > 0; o >>= 1) mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, o));
-      const float e0 = expf(a0 - mx), e1 = expf(a1 - mx);
-      float sum = e0 + e1;
-#pragma unroll
-      for (int o = 16; o > 0; o >>= 1) sum += __shfl_xor_sync(0xffffffffu, sum, o);
-      const float inv = 1.0f / sum;
-      ss[r * 65 + lane] = e0 * inv;
-      ss[r * 65 + lane + 32] = e1 * inv;
-    }
-  }
-  __syncthreads();
-  {  // P V: thread -> 4 q x 4 d
-    const int tq = tid / 8, td = tid % 8;
-    float acc[4][4];
-#pragma unroll
-    for (int a = 0; a < 4; ++a)
-#pragma unroll
-      for (int c = 0; c < 4; ++c) acc[a][c] = 0.f;
-    for (int j = 0; j < 64; ++j) {
-      float pa[4], vb[4];
-#pragma unroll
-      for (int a = 0; a < 4; ++a) pa[a] = ss[(tq * 4 + a) * 65 + j];
-#pragma unroll
-      for (int c = 0; c < 4; ++c) vb[c] = sv[j * 32 + td * 4 + c];
-#pragma unroll
-      for (int a = 0; a < 4; ++a)
-#pragma unroll
-        for (int c = 0; c < 4; ++c) acc[a][c] = fmaf(pa[a], vb[c], acc[a][c]);
-    }
-#pragma unroll
-    for (int a = 0; a < 4; ++a) {
-      const int t = tq * 4 + a;
-      const int64_t pix = (static_cast<int64_t>(b) * h + wy * 8 + t / 8) * w + wx * 8 + t % 8;
-      uint2 u;
-      u.x = pack16x2<BF16>(acc[a][0], acc[a][1]);
-      u.y = pack16x2<BF16>(acc[a][2], acc[a][3]);
-      *reinterpret_cast<uint2*>(out + pix * 128 + head * 32 + td * 4) = u;
-    }
-  }
-}
-
 // CAB channel attention, part 1: per-image channel means of x[NB, HW, C] (16-bit) -> mean[NB, C] fp32
 // (nn.AdaptiveAvgPool2d(1), iggt/heads/window_sa.py:26-38).  Grid (NB, chunks); atomics on a zeroed buffer.
 template <bool BF16>
@@ -387,13 +169,6 @@ inline unsigned grid_cap(int64_t total, int threads = 256) {
 
 using namespace iggt;
 
-namespace {
-int winattn_tc() {
-  static const int v = [] { const char* e = getenv("IGGT_WINATTN_TC"); return e ? atoi(e) : 1; }();
-  return v;
-}
-}  // namespace
-
 extern "C" int iggt_layernorm16(const void* x, void* y, int64_t rows, int C, const float* w, const float* b,
                                 float eps, int dtype, iggt_stream_t stream) {
   if (rows <= 0) return 0;
@@ -423,19 +198,12 @@ extern "C" int iggt_ocab_attention(const void* q, const void* k, const void* v, 
   if (NB <= 0 || (h % 8) || (w % 8)) return -1;
   static DeviceOnce once;
   if (once.first()) {
-    cudaFuncSetAttribute(ocab_attention_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, OCAB_SMEM);
-    cudaFuncSetAttribute(ocab_attention_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, OCAB_SMEM);
     cudaFuncSetAttribute(ocab_attention_tc_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, OA_SMEM);
     cudaFuncSetAttribute(ocab_attention_tc_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, OA_SMEM);
   }
   const unsigned grid = static_cast<unsigned>(NB) * (h / 8) * (w / 8) * 4;
-  if (winattn_tc()) {      // tensor-core kernel (winattn.cuh); IGGT_WINATTN_TC=0 selects the scalar fp32 kernel below
-    if (dtype) ocab_attention_tc_kernel<true><<<grid, 128, OA_SMEM, (cudaStream_t)stream>>>((const uint16_t*)q, (const uint16_t*)k, (const uint16_t*)v, table, rpi, (uint16_t*)out, h, w);
-    else ocab_attention_tc_kernel<false><<<grid, 128, OA_SMEM, (cudaStream_t)stream>>>((const uint16_t*)q, (const uint16_t*)k, (const uint16_t*)v, table, rpi, (uint16_t*)out, h, w);
-    return (int)cudaGetLastError();
-  }
-  if (dtype) ocab_attention_kernel<true><<<grid, 256, OCAB_SMEM, (cudaStream_t)stream>>>((const uint16_t*)q, (const uint16_t*)k, (const uint16_t*)v, table, rpi, (uint16_t*)out, h, w);
-  else ocab_attention_kernel<false><<<grid, 256, OCAB_SMEM, (cudaStream_t)stream>>>((const uint16_t*)q, (const uint16_t*)k, (const uint16_t*)v, table, rpi, (uint16_t*)out, h, w);
+  if (dtype) ocab_attention_tc_kernel<true><<<grid, 128, OA_SMEM, (cudaStream_t)stream>>>((const uint16_t*)q, (const uint16_t*)k, (const uint16_t*)v, table, rpi, (uint16_t*)out, h, w);
+  else ocab_attention_tc_kernel<false><<<grid, 128, OA_SMEM, (cudaStream_t)stream>>>((const uint16_t*)q, (const uint16_t*)k, (const uint16_t*)v, table, rpi, (uint16_t*)out, h, w);
   return (int)cudaGetLastError();
 }
 
@@ -443,13 +211,8 @@ extern "C" int iggt_window_attention(const void* qkv, void* out, int NB, int h, 
                                      iggt_stream_t stream) {
   if (NB <= 0 || (h % 8) || (w % 8)) return -1;
   const unsigned grid = static_cast<unsigned>(NB) * (h / 8) * (w / 8) * 4;
-  if (winattn_tc()) {
-    if (dtype) window_attention_tc_kernel<true><<<grid, 128, 0, (cudaStream_t)stream>>>((const uint16_t*)qkv, (uint16_t*)out, h, w);
-    else window_attention_tc_kernel<false><<<grid, 128, 0, (cudaStream_t)stream>>>((const uint16_t*)qkv, (uint16_t*)out, h, w);
-    return (int)cudaGetLastError();
-  }
-  if (dtype) window_attention_kernel<true><<<grid, 128, 0, (cudaStream_t)stream>>>((const uint16_t*)qkv, (uint16_t*)out, h, w);
-  else window_attention_kernel<false><<<grid, 128, 0, (cudaStream_t)stream>>>((const uint16_t*)qkv, (uint16_t*)out, h, w);
+  if (dtype) window_attention_tc_kernel<true><<<grid, 128, 0, (cudaStream_t)stream>>>((const uint16_t*)qkv, (uint16_t*)out, h, w);
+  else window_attention_tc_kernel<false><<<grid, 128, 0, (cudaStream_t)stream>>>((const uint16_t*)qkv, (uint16_t*)out, h, w);
   return (int)cudaGetLastError();
 }
 

@@ -342,29 +342,4 @@ __device__ __forceinline__ float2 gelu_fast2(float2 x) {
 }
 
 
-// Exact-erf GELU with ONE MUFU per element: erfc(z) = 2^(z * q(z)) for z = |x| / sqrt(2) in [0, 4.3] (q: degree-6
-// least-squares fit of log2(erfc(z)) / z, max error 3e-5 in log2 units), so
-//   gelu(x) = 0.5 x + 0.5 |x| (1 - erfc(z)) = hx - na + na * e,   na = -|hx|,  e = erfc(z),  hx = x / 2.
-// Absolute error <= 1.6e-6, relative error <= 2.1e-5 wherever the result is an fp16 normal (the result is rounded to
-// 16 bit right after, half an fp16 ulp = 2.4e-4).  2 MUFU per pair, against 4 for gelu_fast2 (reciprocal + exponential).
-__device__ __forceinline__ float2 gelu_erfc2(float2 x) {
-  const float2 hx = fmul2(x, make_float2(0.5f, 0.5f));
-  const float2 na = make_float2(__uint_as_float(__float_as_uint(hx.x) | 0x80000000u),
-                                __uint_as_float(__float_as_uint(hx.y) | 0x80000000u));
-  float2 z = fmul2(na, make_float2(-1.4142135623730951f, -1.4142135623730951f));          // |x| / sqrt(2)
-  z.x = fminf(z.x, 4.3f);
-  z.y = fminf(z.y, 4.3f);
-  float2 q = ffma2(make_float2(-1.5555357094854116e-05f, -1.5555357094854116e-05f), z,
-                   make_float2(0.0004183394485153258f, 0.0004183394485153258f));
-  q = ffma2(q, z, make_float2(-0.0048510609194636345f, -0.0048510609194636345f));
-  q = ffma2(q, z, make_float2(0.03291909396648407f, 0.03291909396648407f));
-  q = ffma2(q, z, make_float2(-0.1511300802230835f, -0.1511300802230835f));
-  q = ffma2(q, z, make_float2(-0.9178327322006226f, -0.9178327322006226f));
-  q = ffma2(q, z, make_float2(-1.6279296875f, -1.6279296875f));
-  const float2 pz = fmul2(q, z);
-  const float2 e = make_float2(ex2_approx(pz.x), ex2_approx(pz.y));
-  const float2 s = ffma2(na, make_float2(-1.0f, -1.0f), hx);                                // hx + |hx|
-  return ffma2(na, e, s);
-}
-
 }  // namespace iggt

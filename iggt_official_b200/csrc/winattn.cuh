@@ -4,10 +4,9 @@
 //   HAB   (iggt/heads/window_sa.py:201-227 + heads/block.py:113-130): 64 x 64 x d = 32 per (window, head).
 // One CTA of 4 warps per (image, window, head); warp w owns query rows [16 w, 16 w + 16): S = Q K^T in registers (C
 // fragments), softmax over the fragment rows (quad shuffles), P re-used as the A operand of P V without leaving registers
-// - split into hi + lo 16-bit operands so that the probabilities keep fp32-like precision (the scalar kernels this
-// replaces kept P in fp32) - and V consumed through ldmatrix.trans.  K / V / Q tiles are staged in shared memory with
-// 16-byte rows padded by 16 bytes (bank-conflict-free fragment loads); K / V arrive as 16-byte vectors (the scalar
-// kernels issued one 2-byte load per element).
+// - split into hi + lo 16-bit operands so that the probabilities keep fp32-like precision - and V consumed through
+// ldmatrix.trans.  K / V / Q tiles are staged in shared memory with 16-byte rows padded by 16 bytes (bank-conflict-free
+// fragment loads); K / V arrive as 16-byte vectors.
 #pragma once
 #include "ptx.cuh"
 

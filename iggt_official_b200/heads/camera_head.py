@@ -4,20 +4,17 @@
 M = B*S rows of width 2048 against 216 M parameters: every Linear is a weight stream (fp32 activations, 16-bit
 weights, fp32 accumulate).  For B*S <= 16 the whole head - 4 iterations x (embed, AdaLN, 4 blocks, pose branch) - is ONE
 persistent launch (`iggt_camera_head`, csrc/camera.cu: the producer warp streams weights across phase boundaries, a
-device-wide barrier separates the ~27 phases of an iteration).  Scenes of more than 16 views, devices with fewer than
-128 SMs (an H100 PCIe, a MIG slice) and IGGT_CAMERA_FUSED=0 run layer by layer: `iggt_skinny_gemm`,
-`iggt_small_attention`, `iggt_layernorm`, with the AdaLN modulate in torch arithmetic.
+device-wide barrier separates the ~27 phases of an iteration).  Scenes of more than 16 views and devices with fewer
+than 128 SMs (an H100 PCIe, a MIG slice) run layer by layer: `iggt_skinny_gemm`, `iggt_small_attention`,
+`iggt_layernorm`, with the AdaLN modulate in torch arithmetic.
 """
 import ctypes
-import os
 from typing import List
 
 import torch
 
 from .. import _lib, ops
 from ..layout import Node
-
-FUSED = os.environ.get("IGGT_CAMERA_FUSED", "1") != "0"
 
 DIM = 2048
 HEADS = 16
@@ -135,7 +132,7 @@ class CameraHead(Node):
         dt = compute_dtype or (torch.get_autocast_dtype("cuda") if torch.is_autocast_enabled("cuda") else torch.float16)
         pk = self._packed(dt, dev)
         M = B * S
-        if FUSED and S <= 16 and camera_tokens.is_cuda and _sm_count(dev) >= FUSED_MIN_SMS:
+        if S <= 16 and camera_tokens.is_cuda and _sm_count(dev) >= FUSED_MIN_SMS:
             rows = camera_tokens.reshape(M, C)                    # a strided view of tokens[:, :, 0]: no copy
             if rows.dtype != torch.float32 or rows.stride(1) != 1:
                 rows = rows.float().contiguous()
@@ -149,6 +146,13 @@ class CameraHead(Node):
                 poses = torch.cat([ops.camera_head(pk["cstruct"], pk, rows[b0 * S:(b0 + per) * S], min(per, B - b0), S,
                                                    num_iterations, dt) for b0 in range(0, B, per)], 1)
             return [poses[i].view(B, S, 9) for i in range(num_iterations)]
+        return self._layers(camera_tokens, pk, num_iterations)
+
+    def _layers(self, camera_tokens, pk, num_iterations):
+        """The head layer by layer on camera_tokens [B,S,2048] with the packed weights `pk` of `_packed`."""
+        B, S, C = camera_tokens.shape
+        M = B * S
+        dev = camera_tokens.device
         raw = camera_tokens.reshape(M, C).float().contiguous()
         pt = torch.empty_like(raw)
         ops.layernorm(raw, pk["tok_w"], pk["tok_b"], 1e-5, pt)

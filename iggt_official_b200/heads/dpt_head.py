@@ -15,7 +15,6 @@ All activations are NHWC 16-bit; every convolution runs on the wgmma implicit-GE
 The reference runs these heads in fp32 / TF32 (iggt/models/vggt.py:189); 16-bit operands with fp32 accumulate
 have the same 10-bit mantissa as TF32 when the compute dtype is fp16.
 """
-import os
 from typing import Dict, List, Tuple
 
 import torch
@@ -25,7 +24,6 @@ from ..layout import Node
 
 PATCH = 14
 LAYERS = (4, 11, 17, 23)
-FUSED_TAIL = os.environ.get("IGGT_FUSED_TAIL", "1") != "0"
 
 
 def uv_pos_tables(gh: int, gw: int, ch: int, aspect: float, device) -> Tuple[torch.Tensor, torch.Tensor]:
@@ -61,12 +59,9 @@ def pack_deconv(w, b, dtype, device):
 
 def dense_tail(up, pk, mode):
     """`output_conv2` + head activation on the full-resolution 128-channel map: one launch of the tall-box kernel
-    (csrc/tailconv.cu; the 32-channel map stays in fp32 registers).  IGGT_FUSED_TAIL=0 selects the two-launch form
-    (generic implicit-GEMM conv -> 16-bit map -> per-pixel tail) for A/B checks."""
-    if FUSED_TAIL and up.shape[3] == 128 and pk["oc2a.w"].shape[0] == 32:
-        return ops.dpt_tail_fused(up, pk["oc2a.w"], pk["oc2a.b"], pk["oc2b.w"], pk["oc2b.b"], mode)
-    z = ops.conv_nhwc(up, pk["oc2a.w"], pk["oc2a.b"], act=2)
-    return ops.dpt_tail(z, pk["oc2b.w"], pk["oc2b.b"], mode)
+    (csrc/tailconv.cu; the 32-channel map stays in fp32 registers)."""
+    assert up.shape[3] == 128 and pk["oc2a.w"].shape[0] == 32, (tuple(up.shape), tuple(pk["oc2a.w"].shape))
+    return ops.dpt_tail_fused(up, pk["oc2a.w"], pk["oc2a.b"], pk["oc2b.w"], pk["oc2b.b"], mode)
 
 
 def _f32(p, device):

@@ -270,25 +270,10 @@ def im2col3x3_s2(x):
     return A, ho, wo
 
 
-def dpt_tail(x, w, b, mode):
-    """x [NB,H,W,32] 16-bit -> (main, conf) fp32; mode 0 depth, 1 points, 2 part (channels-first, conf None)."""
-    NB, H, W, _ = x.shape
-    OC = w.shape[0]
-    if mode == 2:
-        main = torch.empty((NB, OC, H, W), dtype=torch.float32, device=x.device)
-        conf = None
-    else:
-        main = torch.empty((NB, H, W, OC - 1), dtype=torch.float32, device=x.device)
-        conf = torch.empty((NB, H, W), dtype=torch.float32, device=x.device)
-    _call(x, "iggt_dpt_tail", 2.0 * NB * H * W * 32 * OC, NB * H * W * (64 + 4 * OC),
-          x.data_ptr(), w.data_ptr(), b.data_ptr(), main.data_ptr(), _ptr(conf), NB, H, W,
-                                   OC, mode, _dt(x), _STREAM)
-    return main, conf
-
-
 def dpt_tail_fused(x, wp, bias, w2, b2, mode):
     """x [NB,H,W,128] 16-bit NHWC -> 3x3 conv (wp [32, 9*128] tap-major) + bias + ReLU -> 1x1 (w2 [OC,32] fp32) ->
-    head activation, one launch (csrc/tailconv.cu).  Returns (main, conf) like `dpt_tail`."""
+    head activation, one launch (csrc/tailconv.cu).  Returns (main, conf) fp32: mode 0 depth, 1 points, 2 part
+    (channels-first [NB, OC, H, W], conf None)."""
     assert x.is_cuda and x.dim() == 4 and x.is_contiguous() and x.shape[3] == 128
     assert wp.shape == (32, 9 * 128) and wp.is_contiguous() and wp.dtype == x.dtype
     NB, H, W, _ = x.shape

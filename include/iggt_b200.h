@@ -141,17 +141,11 @@ int iggt_deconv_shuffle(const void* y, void* out, int NB, int h, int w, int C, i
  * Replaces the gather half of iggt/heads/dpt_head.py:94-97. */
 int iggt_im2col3x3_s2(const void* x, void* A, int NB, int h, int w, int C, iggt_stream_t stream);
 
-/* Per-pixel 1x1 conv 32 -> OC (fp32 weights w[OC][32], b[OC]) + head activation on x[NB,H,W,32].
- * mode 0 (depth): main[NB,H,W,OC-1] = exp, conf[NB,H,W] = 1+exp;  mode 1 (points): sign*expm1|.|;
- * mode 2 (part_feat): raw, channels-first main[NB,OC,H,W].
- * Replaces iggt/heads/dpt_head.py:264-265 + iggt/heads/head_act.py:61-125, part_head.py:240-243. */
-int iggt_dpt_tail(const void* x, const float* w, const float* b, float* out_main, float* out_conf, int NB,
-                  int H, int W, int OC, int mode, int dtype, iggt_stream_t stream);
-
 /* The dense heads' last stage in one launch: 3x3 conv 128 -> 32 (pad 1, weights Wp[32][9*128] tap-major 16-bit,
- * bias[32]) + ReLU + 1x1 conv 32 -> OC in fp32 (w2[OC][32], b2[OC]) + the head activation of iggt_dpt_tail
- * (mode 0 / 1 / 2), x = [NB,H,W,128] 16-bit NHWC.  The 32-channel map never leaves registers.  With w2 == NULL the
- * ReLU map is stored instead (out16 [NB,H,W,32] 16-bit) - the unfused form, kept for A/B checks.
+ * bias[32]) + ReLU + 1x1 conv 32 -> OC in fp32 (w2[OC][32], b2[OC]) + head activation, x = [NB,H,W,128] 16-bit NHWC.
+ * mode 0 (depth): main[NB,H,W,OC-1] = exp, conf[NB,H,W] = 1+exp;  mode 1 (points): sign*expm1|.|;
+ * mode 2 (part_feat): raw, channels-first main[NB,OC,H,W].  The 32-channel map never leaves registers.  With
+ * w2 == NULL the ReLU map is stored instead (out16 [NB,H,W,32] 16-bit), so that the conv half can be checked alone.
  * Replaces iggt/heads/dpt_head.py:120-126 (`output_conv2`) + :264-265 + iggt/heads/head_act.py:61-125, and
  * iggt/heads/part_head.py:240-243. */
 int iggt_dpt_tail_fused(const void* x, const void* Wp, const float* bias, const float* w2, const float* b2,

@@ -1,5 +1,5 @@
-"""Condense an `ncu --page raw --csv` dump (one row per profiled launch; scripts/gpu_r2a.sh writes it on the GPU box,
-because the .ncu-rep of ~50 kernels with the full metric set is >100 MB) into the per-kernel table kept under profiles/:
+"""Condense an `ncu --page raw --csv` dump (one row per profiled launch; kept instead of the .ncu-rep, which is
+>100 MB for ~50 kernels with the full metric set) into the per-kernel table kept under profiles/:
 duration, DRAM bytes and achieved GB/s against the measured HBM peak, tensor / MUFU / issue utilisation, launch shape.
 
     python scripts/ncu_table.py gpurun_out/r02a_ncu_all_raw.csv profiles/r02a_ncu_all_kernels.csv [targets.log]

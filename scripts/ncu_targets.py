@@ -96,8 +96,6 @@ def targets():
     w2, b2 = rnd(4, 32, dtype=torch.float32, scale=0.2), rnd(4, dtype=torch.float32, scale=0.1)
     t["dpt_tail_fused"] = lambda: ops.dpt_tail_fused(up, wt, bt, w2, b2, 1)
     t["conv_nhwc_tail_generic"] = lambda: ops.conv_nhwc(up, wt, bt, act=2)
-    z = rnd(S, 518, 518, 32)
-    t["dpt_tail"] = lambda: ops.dpt_tail(z, w2, b2, 1)
     y4 = rnd(S * g * g, 16 * 256)
     t["deconv_shuffle"] = lambda: ops.deconv_shuffle(y4, S, g, g, 256, 4)
     f37 = rnd(S, g, g, 1024)

@@ -26,18 +26,11 @@ def setup():
 @pytest.mark.parametrize("dtype", [torch.float16, torch.bfloat16])
 @pytest.mark.parametrize("B,S", [(1, 8), (1, 3), (2, 4), (1, 1), (1, 13), (2, 8), (4, 4), (4, 16), (5, 3)])
 def test_fused_camera_head_matches_layer_path_and_oracle(setup, dtype, B, S):
-    from iggt_official_b200.heads import camera_head as CH
     from oracle import ref_model
     head, sd = setup
     tok = _tokens(B, S, B * 100 + S).cuda()
-    toks = [None] * 23 + [tok]
-    CH.FUSED = True
-    fused = head(toks, compute_dtype=dtype)
-    CH.FUSED = False
-    try:
-        layer = head(toks, compute_dtype=dtype)
-    finally:
-        CH.FUSED = True
+    fused = head([None] * 23 + [tok], compute_dtype=dtype)
+    layer = head._layers(tok[:, :, 0], head._packed(dtype, tok.device), 4)
     torch.cuda.synchronize()
     assert len(fused) == 4 and fused[0].shape == (B, S, 9) and fused[0].dtype == torch.float32
     f, l = torch.stack(fused).cpu(), torch.stack(layer).cpu()

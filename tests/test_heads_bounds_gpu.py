@@ -329,23 +329,6 @@ def test_dpt_tail_fused(ops, dtype, NB, H, W, OC, mode):
             _check_tail(main, conf, o64, A, mode, 2.0 ** -18, f"fused tail {NB}x{H}x{W} mode {mode}"))
 
 
-@pytest.mark.parametrize("dtype", DTYPES)
-@pytest.mark.parametrize("NB,H,W", [(2, 9, 11), (1, 518, 518)])
-@pytest.mark.parametrize("OC,mode", [(2, 0), (4, 1), (8, 2)])
-def test_dpt_tail(ops, dtype, NB, H, W, OC, mode):
-    """1x1 32 -> OC in fp32: 32 sequential fmaf from the bias -> |o - o64| <= 32 * 2^-24 A = 2^-19 A."""
-    g = torch.Generator(device="cuda").manual_seed(29 + H)
-    x = (torch.randn(NB, H, W, 32, device="cuda", generator=g) * 2).to(dtype)
-    w = torch.randn(OC, 32, device="cuda", generator=g) / 2
-    b = torch.randn(OC, device="cuda", generator=g) * 0.5
-    main, conf = ops.dpt_tail(x, w, b, mode)
-    torch.cuda.synchronize()
-    o64 = x.double() @ w.double().t() + b.double()
-    A = x.double().abs() @ w.double().abs().t() + b.double().abs()
-    _report(f"dpt_tail {dtype} {NB}x{H}x{W} mode {mode}",
-            _check_tail(main, conf, o64, A, mode, 2.0 ** -19, f"tail {NB}x{H}x{W} mode {mode}"))
-
-
 def _one_hot_tail_inputs(dtype, vals):
     """Inputs for which o is exact: channel 0 of x carries `vals`, the 1x1 (and conv) weights pick it with weight 1, every
     other weight and bias is 0 - the sums then add exact zeros."""
@@ -356,37 +339,33 @@ def _one_hot_tail_inputs(dtype, vals):
 
 
 @pytest.mark.parametrize("dtype", DTYPES)
-@pytest.mark.parametrize("fused", [False, True])
-def test_dpt_tail_expm1_near_zero_and_overflow(ops, dtype, fused):
+@pytest.mark.parametrize("mode,OC", [(0, 2), (1, 4)])
+def test_dpt_tail_expm1_near_zero_and_overflow(ops, dtype, mode, OC):
     """sign * expm1(|o|) keeps its relative accuracy near 0 (expm1f: <= 2 ulp, 2^-22 |r|; exp(o) - 1 would be off by
     2^-24 absolute, thousands of ulp at o = 2^-20), exp(o) and 1 + exp(o) within 2^-22 relative, and o above
     log(FLT_MAX) = 88.72 gives inf at exactly those positions."""
     vals = torch.cat([2.0 ** -torch.arange(1, 24, dtype=torch.float64, device="cuda"),
                       torch.tensor([0.0, 3.0, 40.0, 88.0, 89.0, 100.0, 65000.0 if dtype == torch.float16 else 1e30],
                                    dtype=torch.float64, device="cuda")])
-    for mode, OC in ((0, 2), (1, 4)):
-        x = _one_hot_tail_inputs(dtype, vals)
-        o_exact = x[0, 0, :, 0].double()
-        w2 = torch.zeros(OC, 32, device="cuda")
-        w2[:, 0] = 1.0
-        b2 = torch.zeros(OC, device="cuda")
-        if fused:
-            wp = torch.zeros(32, 9 * 128, device="cuda", dtype=dtype)
-            wp[0, 4 * 128] = 1.0                   # centre tap, channel 0 -> conv channel 0
-            main, conf = ops.dpt_tail_fused(x, wp, torch.zeros(32, device="cuda"), w2, b2, mode)
-        else:
-            main, conf = ops.dpt_tail(x[..., :32].contiguous(), w2, b2, mode)
-        torch.cuda.synchronize()
-        o = o_exact.view(1, 1, -1, 1).expand(1, 1, o_exact.numel(), OC - 1)
-        ref = torch.exp(o) if mode == 0 else torch.expm1(o)
-        fin = torch.isfinite(ref) & (ref < 3.0e38)
-        assert torch.equal(torch.isinf(main), ~fin), f"mode {mode}: inf positions differ"
-        w = check32(main[fin], ref[fin], ref[fin].abs(), 2.0 ** -22, what=f"mode {mode} activation")
-        cref = 1 + torch.exp(o_exact.view(1, 1, -1))
-        cfin = cref < 3.0e38
-        assert torch.equal(torch.isinf(conf), ~cfin)
-        wc = check32(conf[cfin], cref[cfin], cref[cfin], 2.0 ** -22 + U24, what=f"mode {mode} conf")
-        _report(f"tail exact-o {dtype} fused={fused} mode {mode}", w, wc)
+    x = _one_hot_tail_inputs(dtype, vals)
+    o_exact = x[0, 0, :, 0].double()
+    w2 = torch.zeros(OC, 32, device="cuda")
+    w2[:, 0] = 1.0
+    b2 = torch.zeros(OC, device="cuda")
+    wp = torch.zeros(32, 9 * 128, device="cuda", dtype=dtype)
+    wp[0, 4 * 128] = 1.0                       # centre tap, channel 0 -> conv channel 0
+    main, conf = ops.dpt_tail_fused(x, wp, torch.zeros(32, device="cuda"), w2, b2, mode)
+    torch.cuda.synchronize()
+    o = o_exact.view(1, 1, -1, 1).expand(1, 1, o_exact.numel(), OC - 1)
+    ref = torch.exp(o) if mode == 0 else torch.expm1(o)
+    fin = torch.isfinite(ref) & (ref < 3.0e38)
+    assert torch.equal(torch.isinf(main), ~fin), f"mode {mode}: inf positions differ"
+    w = check32(main[fin], ref[fin], ref[fin].abs(), 2.0 ** -22, what=f"mode {mode} activation")
+    cref = 1 + torch.exp(o_exact.view(1, 1, -1))
+    cfin = cref < 3.0e38
+    assert torch.equal(torch.isinf(conf), ~cfin)
+    wc = check32(conf[cfin], cref[cfin], cref[cfin], 2.0 ** -22 + U24, what=f"mode {mode} conf")
+    _report(f"tail exact-o {dtype} mode {mode}", w, wc)
 
 
 # -------------------------------------------------------------------------------------------- pure permutation kernels

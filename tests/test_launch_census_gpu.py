@@ -84,7 +84,6 @@ COVERED_ELSEWHERE = {
     "deconv_shuffle": "test_heads_bounds_gpu.py::test_deconv_shuffle_bit_exact",
     "im2col3x3_s2": "test_heads_bounds_gpu.py::test_im2col3x3_s2_bit_exact",
     "col2im_k4s2p1": "test_heads_bounds_gpu.py::test_col2im_k4s2p1",
-    "dpt_tail": "test_heads_bounds_gpu.py::test_dpt_tail",
     "skinny_gemm": "test_heads_bounds_gpu.py::test_skinny_gemm",
     "small_attention": "test_heads_bounds_gpu.py::test_small_attention",
     "camera_head": "test_heads_bounds_gpu.py::test_camera_head_phases",

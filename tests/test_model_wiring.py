@@ -19,7 +19,7 @@ from oracle import weights                                                  # no
 EMU = {"gemm_store16": emu_ops.gemm_store16_full, "gemm_store32": emu_ops.gemm_store32, "gemm_resid32": emu_ops.gemm_resid32_full,
        "gemm_qkv": emu_ops.gemm_qkv, "attention": emu_ops.attention, "layernorm": emu_ops.layernorm,
        "layernorm16": emu_ops.layernorm16, "conv_nhwc": emu_ops.conv_nhwc, "upsample_bilinear": emu_ops.upsample_bilinear,
-       "deconv_shuffle": emu_ops.deconv_shuffle, "im2col3x3_s2": emu_ops.im2col3x3_s2, "dpt_tail": emu_ops.dpt_tail, "dpt_tail_fused": emu_ops.dpt_tail_fused,
+       "deconv_shuffle": emu_ops.deconv_shuffle, "im2col3x3_s2": emu_ops.im2col3x3_s2, "dpt_tail_fused": emu_ops.dpt_tail_fused,
        "skinny_gemm": emu_ops.skinny_gemm, "small_attention": emu_ops.small_attention, "patchify": emu_ops.patchify,
        "dino_assemble": emu_ops.dino_assemble, "special_tokens": emu_ops.special_tokens,
        "col2im_k4s2p1": emu_ops.col2im_k4s2p1, "ocab_attention": emu_ops.ocab_attention,
