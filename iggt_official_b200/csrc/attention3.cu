@@ -459,15 +459,11 @@ attention3_merge_kernel(const float* __restrict__ ws_o, const float* __restrict_
 template <bool BF16>
 int launch_attention3(const CUtensorMap& tQ, const CUtensorMap& tK, const CUtensorMap& tV, const Attn3Params& p,
                       cudaStream_t stream) {
-  auto kern = attention3_kernel<BF16>;
-  static DeviceOnce once;
-  if (once.first()) {
-    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, A3_SMEM);
-    if (e != cudaSuccess) { once.reset_current(); return (int)e; }
-  }
+  const cudaError_t e = opt_in_smem<attention3_kernel<BF16>>(A3_SMEM);
+  if (e != cudaSuccess) return (int)e;
   const int sms = device_sm_count();
   const int grid = p.total_items < sms ? p.total_items : sms;
-  return (int)launch_pdl(kern, dim3(grid), dim3(A3_THREADS), A3_SMEM, stream, tQ, tK, tV, p);
+  return (int)launch_pdl(attention3_kernel<BF16>, dim3(grid), dim3(A3_THREADS), A3_SMEM, stream, tQ, tK, tV, p);
 }
 
 }  // namespace iggt
@@ -569,43 +565,43 @@ namespace {
 int attention_launch(const void* q, int64_t ldq, const void* k, int64_t ldk, const void* v, int64_t ldv, void* o,
                      int64_t ldo, int num_seq, int Lq, int Lk, int H, int head_dim, float scale, int dtype, int splits,
                      void* ws, int64_t ws_bytes, cudaStream_t s) {
-  if (head_dim != 64) return -1;
-  if (num_seq <= 0 || Lq <= 0 || Lk <= 0 || H <= 0 || splits < 1) return -1;
-  if ((ldq % 8) || (ldk % 8) || (ldv % 8) || (ldo % 8)) return -2;
-  if (dtype != 0 && dtype != 1) return -3;
-  const TmDtype dt = dtype ? TM_BF16 : TM_F16;
-  CUtensorMap tQ, tK, tV;
-  if (make_tmap_2d(&tQ, dt, q, (uint64_t)num_seq * Lq, (uint64_t)H * 64, ldq, 64, A3_BQ)) return -4;
-  // K and V are 3-D {H*64 columns, Lk rows, num_seq sequences}: the ragged last key tile of a sequence reads zeros past
-  // row Lk (TMA fill), never the next sequence's rows.  The mask gives those keys P = 0, but 0 * V is NaN where V is inf,
-  // so with a 2-D map over all sequences one sequence's output could depend on its neighbour's values.
-  {
-    const uint64_t dims[3] = {(uint64_t)H * 64, (uint64_t)Lk, (uint64_t)num_seq};
-    const uint32_t box[3] = {64, A3_BK, 1};
-    const uint64_t kstr[2] = {(uint64_t)ldk * 2, (uint64_t)Lk * ldk * 2};
-    const uint64_t vstr[2] = {(uint64_t)ldv * 2, (uint64_t)Lk * ldv * 2};
-    if (make_tmap(&tK, dt, 3, k, dims, kstr, box)) return -4;
-    if (make_tmap(&tV, dt, 3, v, dims, vstr, box)) return -4;
-  }
-  Attn3Params p;
-  attn3_shape(p, num_seq, Lq, Lk, H, splits);
-  const int n_kv = (Lk + A3_BK - 1) / A3_BK;
-  if ((p.kv_splits - 1) * p.tiles_per_split >= n_kv) return -5;        // an empty kv range: use iggt_attention_plan's count
-  const int64_t rows = static_cast<int64_t>(num_seq) * Lq;
-  if (p.kv_splits > 1) {
-    const int64_t need = p.kv_splits * rows * H * (A3_D + 2) * 4;
-    if (!ws || ws_bytes < need || (reinterpret_cast<uintptr_t>(ws) & 15)) return -6;
-    p.ws_o = reinterpret_cast<float*>(ws);
-    p.ws_ml = p.ws_o + p.kv_splits * rows * H * A3_D;
-  }
-  p.ldo = ldo; p.o = o;
-  p.scale_log2 = scale * 1.4426950408889634f;
-  const int st = dtype ? launch_attention3<true>(tQ, tK, tV, p, s) : launch_attention3<false>(tQ, tK, tV, p, s);
-  if (st != 0 || p.kv_splits == 1) return st;
-  const int64_t warps = rows * H;
-  const unsigned grid = static_cast<unsigned>((warps + 7) / 8);
-  if (dtype) return (int)launch_pdl(attention3_merge_kernel<true>, dim3(grid), dim3(256), 0, s, (const float*)p.ws_o, (const float*)p.ws_ml, o, ldo, rows, H, p.kv_splits, p.scale_log2);
-  return (int)launch_pdl(attention3_merge_kernel<false>, dim3(grid), dim3(256), 0, s, (const float*)p.ws_o, (const float*)p.ws_ml, o, ldo, rows, H, p.kv_splits, p.scale_log2);
+  return dispatch_dtype(dtype, [&](auto bf16) {
+    if (head_dim != 64) return -1;
+    if (num_seq <= 0 || Lq <= 0 || Lk <= 0 || H <= 0 || splits < 1) return -1;
+    if ((ldq % 8) || (ldk % 8) || (ldv % 8) || (ldo % 8)) return -2;
+    CUtensorMap tQ, tK, tV;
+    if (make_tmap_2d(&tQ, tm16(bf16), q, (uint64_t)num_seq * Lq, (uint64_t)H * 64, ldq, 64, A3_BQ)) return -4;
+    // K and V are 3-D {H*64 columns, Lk rows, num_seq sequences}: the ragged last key tile of a sequence reads zeros
+    // past row Lk (TMA fill), never the next sequence's rows.  The mask gives those keys P = 0, but 0 * V is NaN where V
+    // is inf, so with a 2-D map over all sequences one sequence's output could depend on its neighbour's values.
+    {
+      const uint64_t dims[3] = {(uint64_t)H * 64, (uint64_t)Lk, (uint64_t)num_seq};
+      const uint32_t box[3] = {64, A3_BK, 1};
+      const uint64_t kstr[2] = {(uint64_t)ldk * 2, (uint64_t)Lk * ldk * 2};
+      const uint64_t vstr[2] = {(uint64_t)ldv * 2, (uint64_t)Lk * ldv * 2};
+      if (make_tmap(&tK, tm16(bf16), 3, k, dims, kstr, box)) return -4;
+      if (make_tmap(&tV, tm16(bf16), 3, v, dims, vstr, box)) return -4;
+    }
+    Attn3Params p;
+    attn3_shape(p, num_seq, Lq, Lk, H, splits);
+    const int n_kv = (Lk + A3_BK - 1) / A3_BK;
+    if ((p.kv_splits - 1) * p.tiles_per_split >= n_kv) return -5;      // an empty kv range: use iggt_attention_plan's count
+    const int64_t rows = static_cast<int64_t>(num_seq) * Lq;
+    if (p.kv_splits > 1) {
+      const int64_t need = p.kv_splits * rows * H * (A3_D + 2) * 4;
+      if (!ws || ws_bytes < need || (reinterpret_cast<uintptr_t>(ws) & 15)) return -6;
+      p.ws_o = reinterpret_cast<float*>(ws);
+      p.ws_ml = p.ws_o + p.kv_splits * rows * H * A3_D;
+    }
+    p.ldo = ldo; p.o = o;
+    p.scale_log2 = scale * 1.4426950408889634f;
+    const int st = launch_attention3<bf16>(tQ, tK, tV, p, s);
+    if (st != 0 || p.kv_splits == 1) return st;
+    const int64_t warps = rows * H;
+    const unsigned grid = static_cast<unsigned>((warps + 7) / 8);
+    return (int)launch_pdl(attention3_merge_kernel<bf16>, dim3(grid), dim3(256), 0, s, (const float*)p.ws_o,
+                           (const float*)p.ws_ml, o, ldo, rows, H, p.kv_splits, p.scale_log2);
+  });
 }
 }  // namespace
 

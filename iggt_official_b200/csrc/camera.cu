@@ -108,12 +108,6 @@ __device__ __forceinline__ void cam_split(float x, uint16_t& hi, uint16_t& lo) {
   }
 }
 
-__device__ __forceinline__ float warp_sum_f(float v) {
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-  return v;
-}
-
 // MP = padded row count (8 or 16): xs is [k][MP]
 template <bool BF16, int MP>
 __global__ void __launch_bounds__(CAM_THREADS, 1)
@@ -235,14 +229,14 @@ camera_head_kernel(const __grid_constant__ CamProgram prog) {
                     v[i] = *reinterpret_cast<const float4*>(row + (lane + 32 * i) * 4);
                     s += (v[i].x + v[i].y) + (v[i].z + v[i].w);
                   }
-                  const float mean = warp_sum_f(s) * (1.0f / CAM_DIM);
+                  const float mean = warp_sum(s) * (1.0f / CAM_DIM);
                   float q = 0.f;
 #pragma unroll
                   for (int i = 0; i < CAM_DIM / 128; ++i) {
                     const float a = v[i].x - mean, bq = v[i].y - mean, c = v[i].z - mean, d = v[i].w - mean;
                     q += (a * a + bq * bq) + (c * c + d * d);
                   }
-                  const float rstd = rsqrtf(warp_sum_f(q) * (1.0f / CAM_DIM) + P.ln_eps);
+                  const float rstd = rsqrtf(warp_sum(q) * (1.0f / CAM_DIM) + P.ln_eps);
 #pragma unroll
                   for (int i = 0; i < CAM_DIM / 128; ++i) {
                     const int k = (lane + 32 * i) * 4;
@@ -357,7 +351,7 @@ camera_head_kernel(const __grid_constant__ CamProgram prog) {
           for (int j = 0; j < 16; ++j) {
             if (j < prog.S) {
               const float4 k = *reinterpret_cast<const float4*>(qkv + (b * prog.S + j) * P.ldx + CAM_DIM + h * CAM_HD + lane * 4);
-              s[j] = warp_sum_f(q.x * k.x + q.y * k.y + q.z * k.z + q.w * k.w) * 0.08838834764831845f;   // 128^-0.5
+              s[j] = warp_sum(q.x * k.x + q.y * k.y + q.z * k.z + q.w * k.w) * 0.08838834764831845f;   // 128^-0.5
               mx = fmaxf(mx, s[j]);
             }
           }
@@ -393,11 +387,11 @@ camera_head_kernel(const __grid_constant__ CamProgram prog) {
             v[4 * i] = a.x; v[4 * i + 1] = a.y; v[4 * i + 2] = a.z; v[4 * i + 3] = a.w;
             s += (a.x + a.y) + (a.z + a.w);
           }
-          const float mean = warp_sum_f(s) * (1.0f / CAM_DIM);
+          const float mean = warp_sum(s) * (1.0f / CAM_DIM);
           float q = 0.f;
 #pragma unroll
           for (int i = 0; i < CAM_DIM / 32; ++i) { const float d = v[i] - mean; q += d * d; }
-          const float rstd = rsqrtf(warp_sum_f(q) * (1.0f / CAM_DIM) + P.ln_eps);
+          const float rstd = rsqrtf(warp_sum(q) * (1.0f / CAM_DIM) + P.ln_eps);
 #pragma unroll
           for (int i = 0; i < CAM_DIM / 128; ++i) {
             const int k = (lane + 32 * i) * 4;
@@ -435,121 +429,114 @@ extern "C" int64_t iggt_camera_head_workspace(int M) {
 extern "C" int iggt_camera_head(const iggt_camera_weights* w, const float* tokens, int64_t ld_tokens, float* out,
                                 void* workspace, int64_t ws_bytes, int B, int S, int iters, int dtype,
                                 iggt_stream_t stream) {
-  if (!w || !tokens || !out || !workspace || B <= 0 || S <= 0 || iters <= 0) return -1;
-  const int M = B * S;
-  if (M > 16 || S > 16) return -7;                      // larger batches: the per-layer launches (iggt_skinny_gemm ...)
-  if (dtype != 0 && dtype != 1) return -3;
-  if (ws_bytes < iggt_camera_head_workspace(M) || (reinterpret_cast<uintptr_t>(workspace) & 15) || (ld_tokens % 4)) return -6;
-  cudaStream_t s = (cudaStream_t)stream;
-  CamWs ws;
-  float* p = reinterpret_cast<float*>(workspace);
-  ws.pt = p; p += M * CAM_DIM;
-  ws.ptn = p; p += M * CAM_DIM;
-  ws.e = p; p += M * CAM_DIM;
-  ws.x = p; p += M * CAM_DIM;
-  ws.o = p; p += M * CAM_DIM;
-  ws.mod = p; p += M * 3 * CAM_DIM;
-  ws.qkv = p; p += M * 3 * CAM_DIM;
-  ws.f = p; p += M * 4 * CAM_DIM;
-  ws.hdn = p; p += M * 1024;
-  ws.pred = p; p += M * 16;
-  ws.barrier = reinterpret_cast<unsigned*>((reinterpret_cast<uintptr_t>(p) + 127) & ~static_cast<uintptr_t>(127));
-  cudaError_t e = cudaMemsetAsync(ws.barrier, 0, 4, s);
-  if (e != cudaSuccess) return (int)e;
-  e = cudaMemsetAsync(ws.pred, 0, M * 16 * 4, s);       // columns 9..15 of `pred` are the zero padding of embed_pose's K
-  if (e != cudaSuccess) return (int)e;
+  return dispatch_dtype(dtype, [&](auto bf16) {
+    if (!w || !tokens || !out || !workspace || B <= 0 || S <= 0 || iters <= 0) return -1;
+    const int M = B * S;
+    if (M > 16 || S > 16) return -7;                      // larger batches: the per-layer launches (iggt_skinny_gemm ...)
+    if (ws_bytes < iggt_camera_head_workspace(M) || (reinterpret_cast<uintptr_t>(workspace) & 15) || (ld_tokens % 4)) return -6;
+    cudaStream_t s = (cudaStream_t)stream;
+    CamWs ws;
+    float* p = reinterpret_cast<float*>(workspace);
+    ws.pt = p; p += M * CAM_DIM;
+    ws.ptn = p; p += M * CAM_DIM;
+    ws.e = p; p += M * CAM_DIM;
+    ws.x = p; p += M * CAM_DIM;
+    ws.o = p; p += M * CAM_DIM;
+    ws.mod = p; p += M * 3 * CAM_DIM;
+    ws.qkv = p; p += M * 3 * CAM_DIM;
+    ws.f = p; p += M * 4 * CAM_DIM;
+    ws.hdn = p; p += M * 1024;
+    ws.pred = p; p += M * 16;
+    ws.barrier = reinterpret_cast<unsigned*>((reinterpret_cast<uintptr_t>(p) + 127) & ~static_cast<uintptr_t>(127));
+    cudaError_t e = cudaMemsetAsync(ws.barrier, 0, 4, s);
+    if (e != cudaSuccess) return (int)e;
+    e = cudaMemsetAsync(ws.pred, 0, M * 16 * 4, s);       // columns 9..15 of `pred` are the zero padding of embed_pose's K
+    if (e != cudaSuccess) return (int)e;
 
-  CamProgram prog{};
-  prog.iters = iters; prog.M = M; prog.Mpad = M <= 8 ? 8 : 16; prog.B = B; prog.S = S; prog.barrier = ws.barrier;
-  const TmDtype dt = dtype ? TM_BF16 : TM_F16;
-  int nmaps = 0;
-  // weights [N, K] row-major seen as {64 k, N, K / 64} (128B-swizzled rows of 64 k): one box = 16 columns x 1024 k
-  auto add_map = [&](const void* W, int N, int K) -> int {
-    const int k64 = K < 64 ? K : 64;                       // embed_pose: K = 16
-    uint64_t dims[3] = {(uint64_t)k64, (uint64_t)N, (uint64_t)((K + 63) / 64)};
-    uint64_t str[2] = {(uint64_t)K * 2, (uint64_t)128};
-    uint32_t box[3] = {64, (uint32_t)CAM_COLS, (uint32_t)(CAM_KS / 64)};
-    if (nmaps >= CAM_MAX_MAPS || make_tmap(&prog.maps[nmaps], dt, 3, W, dims, str, box, true)) return -1;
-    return nmaps++;
-  };
-  int np = 0;
-  bool bad = false;
-  auto gemm = [&](const void* W, int N, int K, const float* x, long ldx, const float* bias, float* o, long ldo, int act) -> CamPhase& {
-    CamPhase& P = prog.ph[np++];
-    P = CamPhase{};
-    P.type = PH_GEMM; P.N = N; P.K = K; P.x = x; P.ldx = ldx; P.bias = bias; P.out = o; P.ldo = ldo; P.act = act;
-    P.tm = add_map(W, N, K);
-    if (P.tm < 0) bad = true;
-    return P;
-  };
-  auto ln = [](CamPhase& P, const float* lw, const float* lb, float eps) { P.ln = lw ? 1 : 2; P.ln_w = lw; P.ln_b = lb; P.ln_eps = eps; };
-  {   // pose_tokens = token_norm(tokens[:, :, 0]); adaln_norm(pose_tokens)  (camera_head.py:99-100, :117)
-    CamPhase& P0 = prog.ph[np++]; P0 = CamPhase{};
-    P0.type = PH_LNROWS; P0.x = tokens; P0.ldx = ld_tokens; P0.out = ws.pt; P0.ldo = CAM_DIM; P0.flags = CF_ONCE;
-    ln(P0, w->tok_w, w->tok_b, 1e-5f);
-    CamPhase& P1 = prog.ph[np++]; P1 = CamPhase{};
-    P1.type = PH_LNROWS; P1.x = ws.pt; P1.ldx = CAM_DIM; P1.out = ws.ptn; P1.ldo = CAM_DIM; P1.flags = CF_ONCE;
-    ln(P1, nullptr, nullptr, 1e-6f);
-  }
-  {   // module_input = embed_pose(prev or empty); shift / scale / gate = Linear(SiLU(.))  (camera_head.py:105-115)
-    CamPhase& E = gemm(w->emb_w, CAM_DIM, 16, ws.pred, 16, w->emb_b, ws.e, CAM_DIM, 4);
-    E.flags = CF_EMBED_IN; E.x2 = w->empty;
-    gemm(w->mod_w, 3 * CAM_DIM, CAM_DIM, ws.e, CAM_DIM, w->mod_b, ws.mod, 3 * CAM_DIM, 0);
-    CamPhase& Mo = prog.ph[np++]; Mo = CamPhase{};
-    Mo.type = PH_MODULATE; Mo.x = ws.mod; Mo.ldx = 3 * CAM_DIM; Mo.x2 = ws.ptn; Mo.x3 = ws.pt; Mo.out = ws.x; Mo.ldo = CAM_DIM;
-  }
-  for (int b = 0; b < 4; ++b) {   // trunk blocks (layers/block.py:105-106, LayerScale init 0.01)
-    const auto& k = w->blk[b];
-    CamPhase& Q = gemm(k.qkv_w, 3 * CAM_DIM, CAM_DIM, ws.x, CAM_DIM, k.qkv_b, ws.qkv, 3 * CAM_DIM, 0);
-    ln(Q, k.n1w, k.n1b, 1e-5f);
-    CamPhase& A = prog.ph[np++]; A = CamPhase{};
-    A.type = PH_ATTN; A.x = ws.qkv; A.ldx = 3 * CAM_DIM; A.out = ws.o; A.ldo = CAM_DIM;
-    CamPhase& Pr = gemm(k.proj_w, CAM_DIM, CAM_DIM, ws.o, CAM_DIM, k.proj_b, ws.x, CAM_DIM, 0);
-    Pr.gamma = k.ls1; Pr.resid = ws.x; Pr.ldr = CAM_DIM;
-    CamPhase& F1 = gemm(k.fc1_w, 4 * CAM_DIM, CAM_DIM, ws.x, CAM_DIM, k.fc1_b, ws.f, 4 * CAM_DIM, 1);
-    ln(F1, k.n2w, k.n2b, 1e-5f);
-    CamPhase& F2 = gemm(k.fc2_w, CAM_DIM, 4 * CAM_DIM, ws.f, 4 * CAM_DIM, k.fc2_b, ws.x, CAM_DIM, 0);
-    F2.gamma = k.ls2; F2.resid = ws.x; F2.ldr = CAM_DIM;
-  }
-  {   // pose_branch(trunk_norm(.)) and the accumulation / activation  (camera_head.py:124-139)
-    CamPhase& B1 = gemm(w->pb1_w, 1024, CAM_DIM, ws.x, CAM_DIM, w->pb1_b, ws.hdn, 1024, 1);
-    ln(B1, w->trk_w, w->trk_b, 1e-5f);
-    CamPhase& B2 = gemm(w->pb2_w, 9, 1024, ws.hdn, 1024, w->pb2_b, ws.pred, 16, 0);
-    B2.flags = CF_POSE_OUT; B2.out2 = out;
-  }
-  if (bad || np > CAM_MAX_PHASES) return -4;
-  prog.n_phases = np;
+    CamProgram prog{};
+    prog.iters = iters; prog.M = M; prog.Mpad = M <= 8 ? 8 : 16; prog.B = B; prog.S = S; prog.barrier = ws.barrier;
+    int nmaps = 0;
+    // weights [N, K] row-major seen as {64 k, N, K / 64} (128B-swizzled rows of 64 k): one box = 16 columns x 1024 k
+    auto add_map = [&](const void* W, int N, int K) -> int {
+      const int k64 = K < 64 ? K : 64;                       // embed_pose: K = 16
+      uint64_t dims[3] = {(uint64_t)k64, (uint64_t)N, (uint64_t)((K + 63) / 64)};
+      uint64_t str[2] = {(uint64_t)K * 2, (uint64_t)128};
+      uint32_t box[3] = {64, (uint32_t)CAM_COLS, (uint32_t)(CAM_KS / 64)};
+      if (nmaps >= CAM_MAX_MAPS || make_tmap(&prog.maps[nmaps], tm16(bf16), 3, W, dims, str, box, true)) return -1;
+      return nmaps++;
+    };
+    int np = 0;
+    bool bad = false;
+    auto gemm = [&](const void* W, int N, int K, const float* x, long ldx, const float* bias, float* o, long ldo, int act) -> CamPhase& {
+      CamPhase& P = prog.ph[np++];
+      P = CamPhase{};
+      P.type = PH_GEMM; P.N = N; P.K = K; P.x = x; P.ldx = ldx; P.bias = bias; P.out = o; P.ldo = ldo; P.act = act;
+      P.tm = add_map(W, N, K);
+      if (P.tm < 0) bad = true;
+      return P;
+    };
+    auto ln = [](CamPhase& P, const float* lw, const float* lb, float eps) { P.ln = lw ? 1 : 2; P.ln_w = lw; P.ln_b = lb; P.ln_eps = eps; };
+    {   // pose_tokens = token_norm(tokens[:, :, 0]); adaln_norm(pose_tokens)  (camera_head.py:99-100, :117)
+      CamPhase& P0 = prog.ph[np++]; P0 = CamPhase{};
+      P0.type = PH_LNROWS; P0.x = tokens; P0.ldx = ld_tokens; P0.out = ws.pt; P0.ldo = CAM_DIM; P0.flags = CF_ONCE;
+      ln(P0, w->tok_w, w->tok_b, 1e-5f);
+      CamPhase& P1 = prog.ph[np++]; P1 = CamPhase{};
+      P1.type = PH_LNROWS; P1.x = ws.pt; P1.ldx = CAM_DIM; P1.out = ws.ptn; P1.ldo = CAM_DIM; P1.flags = CF_ONCE;
+      ln(P1, nullptr, nullptr, 1e-6f);
+    }
+    {   // module_input = embed_pose(prev or empty); shift / scale / gate = Linear(SiLU(.))  (camera_head.py:105-115)
+      CamPhase& E = gemm(w->emb_w, CAM_DIM, 16, ws.pred, 16, w->emb_b, ws.e, CAM_DIM, 4);
+      E.flags = CF_EMBED_IN; E.x2 = w->empty;
+      gemm(w->mod_w, 3 * CAM_DIM, CAM_DIM, ws.e, CAM_DIM, w->mod_b, ws.mod, 3 * CAM_DIM, 0);
+      CamPhase& Mo = prog.ph[np++]; Mo = CamPhase{};
+      Mo.type = PH_MODULATE; Mo.x = ws.mod; Mo.ldx = 3 * CAM_DIM; Mo.x2 = ws.ptn; Mo.x3 = ws.pt; Mo.out = ws.x; Mo.ldo = CAM_DIM;
+    }
+    for (int b = 0; b < 4; ++b) {   // trunk blocks (layers/block.py:105-106, LayerScale init 0.01)
+      const auto& k = w->blk[b];
+      CamPhase& Q = gemm(k.qkv_w, 3 * CAM_DIM, CAM_DIM, ws.x, CAM_DIM, k.qkv_b, ws.qkv, 3 * CAM_DIM, 0);
+      ln(Q, k.n1w, k.n1b, 1e-5f);
+      CamPhase& A = prog.ph[np++]; A = CamPhase{};
+      A.type = PH_ATTN; A.x = ws.qkv; A.ldx = 3 * CAM_DIM; A.out = ws.o; A.ldo = CAM_DIM;
+      CamPhase& Pr = gemm(k.proj_w, CAM_DIM, CAM_DIM, ws.o, CAM_DIM, k.proj_b, ws.x, CAM_DIM, 0);
+      Pr.gamma = k.ls1; Pr.resid = ws.x; Pr.ldr = CAM_DIM;
+      CamPhase& F1 = gemm(k.fc1_w, 4 * CAM_DIM, CAM_DIM, ws.x, CAM_DIM, k.fc1_b, ws.f, 4 * CAM_DIM, 1);
+      ln(F1, k.n2w, k.n2b, 1e-5f);
+      CamPhase& F2 = gemm(k.fc2_w, CAM_DIM, 4 * CAM_DIM, ws.f, 4 * CAM_DIM, k.fc2_b, ws.x, CAM_DIM, 0);
+      F2.gamma = k.ls2; F2.resid = ws.x; F2.ldr = CAM_DIM;
+    }
+    {   // pose_branch(trunk_norm(.)) and the accumulation / activation  (camera_head.py:124-139)
+      CamPhase& B1 = gemm(w->pb1_w, 1024, CAM_DIM, ws.x, CAM_DIM, w->pb1_b, ws.hdn, 1024, 1);
+      ln(B1, w->trk_w, w->trk_b, 1e-5f);
+      CamPhase& B2 = gemm(w->pb2_w, 9, 1024, ws.hdn, 1024, w->pb2_b, ws.pred, 16, 0);
+      B2.flags = CF_POSE_OUT; B2.out2 = out;
+    }
+    if (bad || np > CAM_MAX_PHASES) return -4;
+    prog.n_phases = np;
 
-  const int sms = device_sm_count();
-  const int grid = sms >= 128 ? 128 : sms;           // 128 | every tile count of the head (128 / 384 / 512): no ragged wave
-  // the consumers keep at most 4 tiles of a phase in registers (acc[4]) while the producer streams the stages of every
-  // tile it assigns to the CTA: below 128 SMs (fc1: 512 tiles) a CTA would own 5 and the weight ring would fall out of
-  // step, so such devices take the per-layer launches
-  int max_tiles = 0;
-  for (int i = 0; i < np; ++i)
-    if (prog.ph[i].type == PH_GEMM && (prog.ph[i].N + CAM_COLS - 1) / CAM_COLS > max_tiles)
-      max_tiles = (prog.ph[i].N + CAM_COLS - 1) / CAM_COLS;
-  if ((max_tiles + grid - 1) / grid > 4) return -7;
-  void (*kern)(const CamProgram) = nullptr;
-  if (prog.Mpad == 8) kern = dtype ? camera_head_kernel<true, 8> : camera_head_kernel<false, 8>;
-  else kern = dtype ? camera_head_kernel<true, 16> : camera_head_kernel<false, 16>;
-  static DeviceOnce once;
-  if (once.first()) {
-    cudaFuncSetAttribute(camera_head_kernel<true, 8>, cudaFuncAttributeMaxDynamicSharedMemorySize, CAM_SMEM);
-    cudaFuncSetAttribute(camera_head_kernel<false, 8>, cudaFuncAttributeMaxDynamicSharedMemorySize, CAM_SMEM);
-    cudaFuncSetAttribute(camera_head_kernel<true, 16>, cudaFuncAttributeMaxDynamicSharedMemorySize, CAM_SMEM);
-    cudaFuncSetAttribute(camera_head_kernel<false, 16>, cudaFuncAttributeMaxDynamicSharedMemorySize, CAM_SMEM);
-  }
-  // every CTA must be resident for the device-wide barrier: a cooperative launch guarantees it (or fails loudly)
-  cudaLaunchConfig_t cfg{};
-  cfg.gridDim = dim3(grid);
-  cfg.blockDim = dim3(CAM_THREADS);
-  cfg.dynamicSmemBytes = CAM_SMEM;
-  cfg.stream = s;
-  cudaLaunchAttribute at[1];
-  at[0].id = cudaLaunchAttributeCooperative;
-  at[0].val.cooperative = 1;
-  cfg.attrs = at;
-  cfg.numAttrs = 1;
-  return (int)cudaLaunchKernelEx(&cfg, kern, prog);
+    const int sms = device_sm_count();
+    const int grid = sms >= 128 ? 128 : sms;           // 128 | every tile count of the head (128 / 384 / 512): no ragged wave
+    // the consumers keep at most 4 tiles of a phase in registers (acc[4]) while the producer streams the stages of every
+    // tile it assigns to the CTA: below 128 SMs (fc1: 512 tiles) a CTA would own 5 and the weight ring would fall out of
+    // step, so such devices take the per-layer launches
+    int max_tiles = 0;
+    for (int i = 0; i < np; ++i)
+      if (prog.ph[i].type == PH_GEMM && (prog.ph[i].N + CAM_COLS - 1) / CAM_COLS > max_tiles)
+        max_tiles = (prog.ph[i].N + CAM_COLS - 1) / CAM_COLS;
+    if ((max_tiles + grid - 1) / grid > 4) return -7;
+    void (*kern)(const CamProgram) = prog.Mpad == 8 ? camera_head_kernel<bf16, 8> : camera_head_kernel<bf16, 16>;
+    e = opt_in_smem<camera_head_kernel<bf16, 8>, camera_head_kernel<bf16, 16>>(CAM_SMEM);
+    if (e != cudaSuccess) return (int)e;
+    // every CTA must be resident for the device-wide barrier: a cooperative launch guarantees it (or fails loudly)
+    cudaLaunchConfig_t cfg{};
+    cfg.gridDim = dim3(grid);
+    cfg.blockDim = dim3(CAM_THREADS);
+    cfg.dynamicSmemBytes = CAM_SMEM;
+    cfg.stream = s;
+    cudaLaunchAttribute at[1];
+    at[0].id = cudaLaunchAttributeCooperative;
+    at[0].val.cooperative = 1;
+    cfg.attrs = at;
+    cfg.numAttrs = 1;
+    return (int)cudaLaunchKernelEx(&cfg, kern, prog);
+  });
 }

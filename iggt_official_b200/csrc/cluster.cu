@@ -511,12 +511,8 @@ extern "C" int iggt_cluster_core(const float* sorted8, const float* box, int64_t
                                  iggt_stream_t stream) {
   if (!sorted8 || !box || !core2 || n <= 0 || n >= (1LL << 31) || k < 1 || k > CL_KMAX || k >= n) return -1;
   const size_t smem = static_cast<size_t>(k) * CL_CTA * sizeof(float);
-  static DeviceOnce once;                               // the opt-in holds for the current device only
-  if (once.first()) {
-    const cudaError_t e = cudaFuncSetAttribute(cl_core_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                               CL_KMAX * CL_CTA * static_cast<int>(sizeof(float)));
-    if (e != cudaSuccess) { once.reset_current(); return (int)e; }
-  }
+  const cudaError_t e = opt_in_smem<cl_core_kernel>(CL_KMAX * CL_CTA * sizeof(float));
+  if (e != cudaSuccess) return (int)e;
   const int nb = static_cast<int>((n + CL_TILE - 1) / CL_TILE);
   cl_core_kernel<<<static_cast<unsigned>((n + CL_CTA - 1) / CL_CTA), CL_CTA, smem, (cudaStream_t)stream>>>(
       reinterpret_cast<const float4*>(sorted8), box, n, nb, k, core2);

@@ -7,12 +7,6 @@
 
 namespace iggt {
 
-__device__ __forceinline__ float warp_sum(float v) {
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-  return v;
-}
-
 // One warp per row. Row r_out = g*rows_out + i  <-  r_in = g*rows_in + in_off + i  (i < rows_out).
 // VEC = C / 128 float4 per lane.
 template <int VEC, bool OUT32, bool BF16>
@@ -87,10 +81,7 @@ patchify_kernel(const float* __restrict__ img, uint16_t* __restrict__ A, int NI,
       const float px = __ldg(img + ((static_cast<int64_t>(n) * 3 + c) * H + pr * 14 + ky) * W + pc * 14 + kx);
       val = (px - mean[c]) / stdv[c];
     }
-    uint16_t h;
-    if constexpr (BF16) { __nv_bfloat16 t = __float2bfloat16_rn(val); h = *reinterpret_cast<uint16_t*>(&t); }
-    else { __half t = __float2half_rn(val); h = *reinterpret_cast<uint16_t*>(&t); }
-    A[patch * KP + k] = h;
+    A[patch * KP + k] = st16<BF16>(val);
   }
 }
 
@@ -116,16 +107,8 @@ dino_assemble_kernel(const uint16_t* __restrict__ pe, const float* __restrict__ 
       const int pidx = t - 1 - R;
       const uint2 u = __ldg(reinterpret_cast<const uint2*>(pe + (static_cast<int64_t>(n) * P + pidx) * C + c));
       const float4 b = __ldg(reinterpret_cast<const float4*>(pos + static_cast<int64_t>(1 + pidx) * C + c));
-      float f0, f1, f2, f3;
-      if constexpr (BF16) {
-        f0 = __uint_as_float(u.x << 16); f1 = __uint_as_float(u.x & 0xFFFF0000u);
-        f2 = __uint_as_float(u.y << 16); f3 = __uint_as_float(u.y & 0xFFFF0000u);
-      } else {
-        const __half2 h0 = *reinterpret_cast<const __half2*>(&u.x);
-        const __half2 h1 = *reinterpret_cast<const __half2*>(&u.y);
-        f0 = __low2float(h0); f1 = __high2float(h0); f2 = __low2float(h1); f3 = __high2float(h1);
-      }
-      o = make_float4(f0 + b.x, f1 + b.y, f2 + b.z, f3 + b.w);
+      const float2 f01 = cvt16x2<BF16>(u.x), f23 = cvt16x2<BF16>(u.y);
+      o = make_float4(f01.x + b.x, f01.y + b.y, f23.x + b.z, f23.y + b.w);
     }
     *reinterpret_cast<float4*>(x + row * C + c) = o;
   }
@@ -155,6 +138,7 @@ extern "C" int iggt_layernorm(const float* x, int64_t ldx, void* y, int64_t ldy,
                               const float* b, float eps, int64_t groups, int rows_out, int rows_in,
                               int in_off, int out_rows_per_group, int out_off, int out_kind,
                               iggt_stream_t stream) {
+  if (out_kind < 0 || out_kind > 2) return -3;
   if (C != 1024 && C != 2048) return -1;
   if ((ldx % 4) || (ldy % 4)) return -2;
   if (groups <= 0 || rows_out <= 0) return 0;
@@ -179,21 +163,23 @@ extern "C" int iggt_layernorm(const float* x, int64_t ldx, void* y, int64_t ldy,
 
 extern "C" int iggt_patchify(const float* images, void* A, int NI, int H, int W, int KP, int dtype,
                              iggt_stream_t stream) {
-  if (NI <= 0 || (H % 14) || (W % 14) || KP < 588 || (KP % 8)) return -1;
-  const int gh = H / 14, gw = W / 14;
-  const unsigned grid = static_cast<unsigned>(NI) * gh * gw;
-  if (dtype) patchify_kernel<true><<<grid, 256, 0, (cudaStream_t)stream>>>(images, (uint16_t*)A, NI, H, W, gh, gw, KP);
-  else patchify_kernel<false><<<grid, 256, 0, (cudaStream_t)stream>>>(images, (uint16_t*)A, NI, H, W, gh, gw, KP);
-  return (int)cudaGetLastError();
+  return dispatch_dtype(dtype, [&](auto bf16) {
+    if (NI <= 0 || (H % 14) || (W % 14) || KP < 588 || (KP % 8)) return -1;
+    const int gh = H / 14, gw = W / 14;
+    const unsigned grid = static_cast<unsigned>(NI) * gh * gw;
+    patchify_kernel<bf16><<<grid, 256, 0, (cudaStream_t)stream>>>(images, (uint16_t*)A, NI, H, W, gh, gw, KP);
+    return (int)cudaGetLastError();
+  });
 }
 
 extern "C" int iggt_dino_assemble(const void* pe16, const float* cls, const float* reg, const float* pos,
                                   float* x, int NI, int P, int R, int C, int dtype, iggt_stream_t stream) {
-  if (NI <= 0 || P <= 0 || (C % 4)) return -1;
-  const unsigned grid = static_cast<unsigned>(NI) * (1 + R + P);
-  if (dtype) dino_assemble_kernel<true><<<grid, 256, 0, (cudaStream_t)stream>>>((const uint16_t*)pe16, cls, reg, pos, x, P, R, C);
-  else dino_assemble_kernel<false><<<grid, 256, 0, (cudaStream_t)stream>>>((const uint16_t*)pe16, cls, reg, pos, x, P, R, C);
-  return (int)cudaGetLastError();
+  return dispatch_dtype(dtype, [&](auto bf16) {
+    if (NI <= 0 || P <= 0 || (C % 4)) return -1;
+    const unsigned grid = static_cast<unsigned>(NI) * (1 + R + P);
+    dino_assemble_kernel<bf16><<<grid, 256, 0, (cudaStream_t)stream>>>((const uint16_t*)pe16, cls, reg, pos, x, P, R, C);
+    return (int)cudaGetLastError();
+  });
 }
 
 extern "C" int iggt_special_tokens(const float* cam, const float* reg, float* x, int NI, int T, int R,

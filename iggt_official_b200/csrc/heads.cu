@@ -9,37 +9,9 @@
 
 namespace iggt {
 
-template <bool BF16>
-__device__ __forceinline__ void unpack8(const uint4& u, float (&f)[8]) {
-  const uint32_t w[4] = {u.x, u.y, u.z, u.w};
-#pragma unroll
-  for (int j = 0; j < 4; ++j) {
-    if constexpr (BF16) {
-      f[2 * j] = __uint_as_float(w[j] << 16);
-      f[2 * j + 1] = __uint_as_float(w[j] & 0xFFFF0000u);
-    } else {
-      const __half2 h = *reinterpret_cast<const __half2*>(&w[j]);
-      f[2 * j] = __low2float(h);
-      f[2 * j + 1] = __high2float(h);
-    }
-  }
-}
-template <bool BF16>
-__device__ __forceinline__ uint4 pack8(const float (&f)[8]) {
-  uint4 u;
-  u.x = pack16x2<BF16>(f[0], f[1]); u.y = pack16x2<BF16>(f[2], f[3]);
-  u.z = pack16x2<BF16>(f[4], f[5]); u.w = pack16x2<BF16>(f[6], f[7]);
-  return u;
-}
-
 // F.interpolate(mode="bilinear", align_corners=True) on NHWC (iggt/heads/dpt_head.py:251-256,478,484-509)
 // + optional pos-embed: channels [0,C/2) get tabx[x][c], [C/2,C) get taby[y][c-C/2]
 // (iggt/heads/dpt_head.py:274-284, iggt/heads/utils.py:11-108; tables are built on the host in float64).
-template <bool BF16>
-__device__ __forceinline__ float2 cvt16x2(uint32_t u) {
-  if constexpr (BF16) return make_float2(__uint_as_float(u << 16), __uint_as_float(u & 0xFFFF0000u));
-  else return __half22float2(*reinterpret_cast<const __half2*>(&u));
-}
 // One CTA per output row (n, oy): the vertical taps / weights are row constants, a thread walks (ox, 8-channel group)
 // items of the row.  Index arithmetic stays 32-bit; the four-tap blend runs on fp32 pairs (same IEEE results as scalar
 // code).
@@ -217,10 +189,7 @@ skinny_gemm_kernel(const __grid_constant__ CUtensorMap tmW, const __grid_constan
 #pragma unroll
   for (int c = 0; c < 4; ++c)
 #pragma unroll
-    for (int m = 0; m < 8; ++m) {
-#pragma unroll
-      for (int o = 16; o > 0; o >>= 1) acc[c][m] += __shfl_xor_sync(0xffffffffu, acc[c][m], o);
-    }
+    for (int m = 0; m < 8; ++m) acc[c][m] = warp_sum(acc[c][m]);
   {
     const int c = lane / 8, m = lane % 8;
     const int n = n0 + warp * 4 + c;
@@ -274,8 +243,7 @@ small_attention_kernel(const float* __restrict__ qkv, float* __restrict__ out, i
     for (int o = 16; o > 0; o >>= 1) mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, o));
     float sum = 0.f;
     for (int j = lane; j < N; j += 32) { const float e = expf(p[j] - mx); p[j] = e; sum += e; }
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) sum += __shfl_xor_sync(0xffffffffu, sum, o);
+    sum = warp_sum(sum);
     __syncwarp();
     const float inv = 1.0f / sum;
     for (int c = lane; c < d; c += 32) {
@@ -287,33 +255,27 @@ small_attention_kernel(const float* __restrict__ qkv, float* __restrict__ out, i
   }
 }
 
-inline unsigned grid_for(int64_t total, int threads = 256) {
-  int64_t g = (total + threads - 1) / threads;
-  const int64_t cap = 132 * 16;
-  return static_cast<unsigned>(g < cap ? (g > 0 ? g : 1) : cap);
-}
-
 }  // namespace iggt
 
 using namespace iggt;
 
 extern "C" int iggt_upsample_bilinear_nhwc(const void* x, void* out, int NB, int h, int w, int H, int W, int C,
                                            const float* tabx, const float* taby, int dtype, iggt_stream_t stream) {
-  if (NB <= 0 || h <= 0 || w <= 0 || H <= 0 || W <= 0 || (C % 16)) return -1;
-  if ((tabx == nullptr) != (taby == nullptr)) return -1;
-  if (static_cast<int64_t>(NB) * H > 0x7fffffff || static_cast<int64_t>(w) * C > 0x7fffffff) return -1;
-  const unsigned rows = static_cast<unsigned>(NB) * H;                 // one CTA per output row
-  if (dtype) upsample_bilinear_kernel<true><<<rows, 256, 0, (cudaStream_t)stream>>>(
-      (const uint16_t*)x, (uint16_t*)out, NB, h, w, H, W, C, tabx, taby);
-  else upsample_bilinear_kernel<false><<<rows, 256, 0, (cudaStream_t)stream>>>(
-      (const uint16_t*)x, (uint16_t*)out, NB, h, w, H, W, C, tabx, taby);
-  return (int)cudaGetLastError();
+  return dispatch_dtype(dtype, [&](auto bf16) {
+    if (NB <= 0 || h <= 0 || w <= 0 || H <= 0 || W <= 0 || (C % 16)) return -1;
+    if ((tabx == nullptr) != (taby == nullptr)) return -1;
+    if (static_cast<int64_t>(NB) * H > 0x7fffffff || static_cast<int64_t>(w) * C > 0x7fffffff) return -1;
+    const unsigned rows = static_cast<unsigned>(NB) * H;                 // one CTA per output row
+    upsample_bilinear_kernel<bf16><<<rows, 256, 0, (cudaStream_t)stream>>>((const uint16_t*)x, (uint16_t*)out, NB, h, w,
+                                                                           H, W, C, tabx, taby);
+    return (int)cudaGetLastError();
+  });
 }
 
 extern "C" int iggt_deconv_shuffle(const void* y, void* out, int NB, int h, int w, int C, int k, iggt_stream_t stream) {
   if (NB <= 0 || (C % 8) || k <= 0) return -1;
   const int64_t total = static_cast<int64_t>(NB) * h * w * k * k * (C / 8);
-  deconv_shuffle_kernel<<<grid_for(total), 256, 0, (cudaStream_t)stream>>>((const uint4*)y, (uint4*)out, NB, h, w, C, k);
+  deconv_shuffle_kernel<<<grid_stride_blocks(total), 256, 0, (cudaStream_t)stream>>>((const uint4*)y, (uint4*)out, NB, h, w, C, k);
   return (int)cudaGetLastError();
 }
 
@@ -321,41 +283,40 @@ extern "C" int iggt_im2col3x3_s2(const void* x, void* A, int NB, int h, int w, i
   if (NB <= 0 || (C % 8)) return -1;
   const int ho = (h - 1) / 2 + 1, wo = (w - 1) / 2 + 1;
   const int64_t total = static_cast<int64_t>(NB) * ho * wo * 9 * (C / 8);
-  im2col_s2_kernel<<<grid_for(total), 256, 0, (cudaStream_t)stream>>>((const uint4*)x, (uint4*)A, NB, h, w, C, ho, wo);
+  im2col_s2_kernel<<<grid_stride_blocks(total), 256, 0, (cudaStream_t)stream>>>((const uint4*)x, (uint4*)A, NB, h, w, C, ho, wo);
   return (int)cudaGetLastError();
 }
 
 extern "C" int iggt_skinny_gemm(const float* x, int64_t ldx, const void* W, int64_t ldw, const float* bias,
                                 const float* gamma, const float* resid, int64_t ldr, float* out, int64_t ldo,
                                 int M, int N, int K, int act, int dtype, iggt_stream_t stream) {
-  if (M <= 0 || M > 32 || N <= 0 || K <= 0 || (K % 8) || (ldx % 4) || (ldw % 8)) return -1;
-  const unsigned grid = (N + SK_COLS - 1) / SK_COLS;
-  cudaStream_t s = (cudaStream_t)stream;
-  static DeviceOnce once;
-  if (once.first()) {
-    cudaFuncSetAttribute(skinny_gemm_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, SK_SMEM);
-    cudaFuncSetAttribute(skinny_gemm_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, SK_SMEM);
-  }
-  CUtensorMap tW;
-  {
-    uint64_t dims[2] = {(uint64_t)K, (uint64_t)N};
-    uint64_t str[1] = {(uint64_t)ldw * 2};
-    uint32_t box[2] = {SK_KC, SK_COLS};
-    if (make_tmap(&tW, dtype ? TM_BF16 : TM_F16, 2, W, dims, str, box, false)) return -4;
-  }
-  for (int m0 = 0; m0 < M; m0 += 8) {   // weights of the later chunks come from L2
-    const int mm = M - m0 < 8 ? M - m0 : 8;
-    const float* rp = resid ? resid + m0 * ldr : nullptr;
-    CUtensorMap tX;
-    uint64_t dims[2] = {(uint64_t)K, (uint64_t)mm};
-    uint64_t str[1] = {(uint64_t)ldx * 4};
-    uint32_t box[2] = {SK_KC, 8};
-    if (make_tmap(&tX, TM_F32, 2, x + m0 * ldx, dims, str, box, false)) return -4;
-    float* op = out + m0 * ldo;
-    if (dtype) launch_pdl(skinny_gemm_kernel<true>, dim3(grid), dim3(288), SK_SMEM, s, tW, tX, bias, gamma, rp, ldr, op, ldo, mm, N, K, act);
-    else launch_pdl(skinny_gemm_kernel<false>, dim3(grid), dim3(288), SK_SMEM, s, tW, tX, bias, gamma, rp, ldr, op, ldo, mm, N, K, act);
-  }
-  return (int)cudaGetLastError();
+  return dispatch_dtype(dtype, [&](auto bf16) {
+    if (M <= 0 || M > 32 || N <= 0 || K <= 0 || (K % 8) || (ldx % 4) || (ldw % 8)) return -1;
+    const unsigned grid = (N + SK_COLS - 1) / SK_COLS;
+    cudaStream_t s = (cudaStream_t)stream;
+    const cudaError_t e = opt_in_smem<skinny_gemm_kernel<bf16>>(SK_SMEM);
+    if (e != cudaSuccess) return (int)e;
+    CUtensorMap tW;
+    {
+      uint64_t dims[2] = {(uint64_t)K, (uint64_t)N};
+      uint64_t str[1] = {(uint64_t)ldw * 2};
+      uint32_t box[2] = {SK_KC, SK_COLS};
+      if (make_tmap(&tW, tm16(bf16), 2, W, dims, str, box, false)) return -4;
+    }
+    for (int m0 = 0; m0 < M; m0 += 8) {   // weights of the later chunks come from L2
+      const int mm = M - m0 < 8 ? M - m0 : 8;
+      const float* rp = resid ? resid + m0 * ldr : nullptr;
+      CUtensorMap tX;
+      uint64_t dims[2] = {(uint64_t)K, (uint64_t)mm};
+      uint64_t str[1] = {(uint64_t)ldx * 4};
+      uint32_t box[2] = {SK_KC, 8};
+      if (make_tmap(&tX, TM_F32, 2, x + m0 * ldx, dims, str, box, false)) return -4;
+      float* op = out + m0 * ldo;
+      launch_pdl(skinny_gemm_kernel<bf16>, dim3(grid), dim3(288), SK_SMEM, s, tW, tX, bias, gamma, rp, ldr, op, ldo, mm, N,
+                 K, act);
+    }
+    return (int)cudaGetLastError();
+  });
 }
 
 extern "C" int iggt_small_attention(const float* qkv, float* out, int B, int N, int H, int d, float scale,
@@ -363,10 +324,8 @@ extern "C" int iggt_small_attention(const float* qkv, float* out, int B, int N, 
   if (B <= 0 || N <= 0 || N > 256 || H <= 0 || d <= 0) return -1;
   const size_t smem = (2 * static_cast<size_t>(N) * d + 4 * N) * sizeof(float);
   if (smem > 200 * 1024) return -1;
-  static DeviceOnce once;
-  if (once.first()) {
-    cudaFuncSetAttribute(small_attention_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
-  }
+  const cudaError_t e = opt_in_smem<small_attention_kernel>(200 * 1024);
+  if (e != cudaSuccess) return (int)e;
   small_attention_kernel<<<B * H, 128, smem, (cudaStream_t)stream>>>(qkv, out, N, H, d, scale);
   return (int)cudaGetLastError();
 }

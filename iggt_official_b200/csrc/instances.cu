@@ -205,15 +205,8 @@ template <int BN>
 int launch_mask_overlaps(const uint8_t* g, int64_t K, int64_t ldg, const uint8_t* pm, int64_t P, int64_t ldp,
                          int64_t n, int64_t* inter, int64_t* gsize, int64_t* psize, cudaStream_t st) {
   using SM = MoSmem<BN>;
-  static DeviceOnce once;
-  if (once.first()) {
-    const cudaError_t e = cudaFuncSetAttribute(mask_overlaps_kernel<BN>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                               SM::TOTAL);
-    if (e != cudaSuccess) {
-      once.reset_current();
-      return (int)e;
-    }
-  }
+  cudaError_t e = opt_in_smem<mask_overlaps_kernel<BN>>(SM::TOTAL);
+  if (e != cudaSuccess) return (int)e;
   CUtensorMap tmG, tmP;
   const uint64_t gdims[2] = {static_cast<uint64_t>(n), static_cast<uint64_t>(K)};
   const uint64_t gstr[1] = {static_cast<uint64_t>(ldg)};
@@ -238,7 +231,7 @@ int launch_mask_overlaps(const uint8_t* g, int64_t K, int64_t ldg, const uint8_t
   prm.gsize = gsize;
   prm.psize = psize;
 
-  cudaError_t e = cudaMemsetAsync(inter, 0, static_cast<size_t>(K * P) * sizeof(int64_t), st);
+  e = cudaMemsetAsync(inter, 0, static_cast<size_t>(K * P) * sizeof(int64_t), st);
   if (e == cudaSuccess) e = cudaMemsetAsync(gsize, 0, static_cast<size_t>(K) * sizeof(int64_t), st);
   if (e == cudaSuccess) e = cudaMemsetAsync(psize, 0, static_cast<size_t>(P) * sizeof(int64_t), st);
   if (e != cudaSuccess) return (int)e;

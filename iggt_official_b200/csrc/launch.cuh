@@ -5,7 +5,10 @@
 // otherwise exposed.  IGGT_PDL=0 falls back to plain stream-ordered launches.
 #pragma once
 #include <cuda_runtime.h>
+#include <stdint.h>
 #include <stdlib.h>
+#include <initializer_list>
+#include <type_traits>
 #include <utility>
 
 namespace iggt {
@@ -21,7 +24,7 @@ inline int current_device() {
   cudaGetDevice(&d);
   return d;
 }
-// `static DeviceOnce once; if (once.first()) { ...configure the kernel on the current device... }`
+// first() is true at the first call on each device, and again after reset_current() on that device
 struct DeviceOnce {
   bool done[kMaxDevices] = {};
   bool first() {
@@ -36,6 +39,22 @@ struct DeviceOnce {
     if (d >= 0 && d < kMaxDevices) done[d] = false;
   }
 };
+// Lets each of `Kernels` use `bytes` of dynamic shared memory on the current device (once per device).  Returns the
+// first failing cudaError_t and forgets the attempt, so the next launch tries again instead of failing with a launch
+// error that hides the cause.
+template <auto... Kernels>
+inline cudaError_t opt_in_smem(size_t bytes) {
+  static DeviceOnce once;
+  if (!once.first()) return cudaSuccess;
+  for (const void* k : {reinterpret_cast<const void*>(Kernels)...}) {
+    const cudaError_t e = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(bytes));
+    if (e != cudaSuccess) {
+      once.reset_current();
+      return e;
+    }
+  }
+  return cudaSuccess;
+}
 inline int device_sm_count() {
   static int n[kMaxDevices] = {};
   const int d = current_device();
@@ -45,6 +64,23 @@ inline int device_sm_count() {
     if (n[d] <= 0) n[d] = 132;
   }
   return n[d];
+}
+
+// Blocks of a grid-stride launch of `threads`-thread blocks over `work` items: one item per thread, at most 16 blocks
+// for each of the H100's 132 SMs.
+constexpr int64_t kGridStrideMaxBlocks = 132 * 16;
+inline unsigned grid_stride_blocks(int64_t work, int threads = 256) {
+  const int64_t g = (work + threads - 1) / threads;
+  return static_cast<unsigned>(g < 1 ? 1 : (g > kGridStrideMaxBlocks ? kGridStrideMaxBlocks : g));
+}
+
+// Calls f(std::true_type{}) for dtype 1 (bf16) or f(std::false_type{}) for dtype 0 (fp16), so a launcher writes each
+// launch once for both element types; any other code returns -3 without calling f.
+template <typename F>
+inline int dispatch_dtype(int dtype, F&& f) {
+  if (dtype == 1) return f(std::true_type{});
+  if (dtype == 0) return f(std::false_type{});
+  return -3;
 }
 
 inline int pdl_enabled() {

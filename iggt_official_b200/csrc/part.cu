@@ -11,17 +11,6 @@
 
 namespace iggt {
 
-template <bool BF16>
-__device__ __forceinline__ float ld16(const uint16_t* p) {
-  if constexpr (BF16) return __uint_as_float(static_cast<uint32_t>(*p) << 16);
-  else return __half2float(__ushort_as_half(*p));
-}
-template <bool BF16>
-__device__ __forceinline__ uint16_t st16(float v) {
-  if constexpr (BF16) { __nv_bfloat16 t = __float2bfloat16_rn(v); return *reinterpret_cast<uint16_t*>(&t); }
-  else { __half t = __float2half_rn(v); return *reinterpret_cast<uint16_t*>(&t); }
-}
-
 // LayerNorm over C in {64,128,256} channels of 16-bit rows (nn.LayerNorm eps 1e-5 of window_sa.py's
 // patch_embed.norm / norm1 / norm2 / norm), fp32 statistics, one warp per row.
 template <bool BF16, int C>
@@ -36,15 +25,11 @@ layernorm16_kernel(const uint16_t* __restrict__ x, uint16_t* __restrict__ y, con
   float s = 0.f;
 #pragma unroll
   for (int i = 0; i < PER; ++i) { v[i] = ld16<BF16>(x + r * C + lane * PER + i); s += v[i]; }
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
-  const float mean = s / C;
+  const float mean = warp_sum(s) / C;
   float q = 0.f;
 #pragma unroll
   for (int i = 0; i < PER; ++i) { const float d = v[i] - mean; q += d * d; }
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) q += __shfl_xor_sync(0xffffffffu, q, o);
-  const float rstd = rsqrtf(q / C + eps);
+  const float rstd = rsqrtf(warp_sum(q) / C + eps);
 #pragma unroll
   for (int i = 0; i < PER; ++i) {
     const int c = lane * PER + i;
@@ -92,10 +77,7 @@ col2im_k4s2p1_kernel(const uint16_t* __restrict__ Y, const float* __restrict__ b
         }
       }
     }
-    uint4 o;
-    o.x = pack16x2<BF16>(acc[0], acc[1]); o.y = pack16x2<BF16>(acc[2], acc[3]);
-    o.z = pack16x2<BF16>(acc[4], acc[5]); o.w = pack16x2<BF16>(acc[6], acc[7]);
-    *reinterpret_cast<uint4*>(out + ((static_cast<int64_t>(n) * H + oy) * W + ox) * C + c8 * 8) = o;
+    *reinterpret_cast<uint4*>(out + ((static_cast<int64_t>(n) * H + oy) * W + ox) * C + c8 * 8) = pack8<BF16>(acc);
   }
 }
 
@@ -152,17 +134,8 @@ se_scale_add_kernel(const uint16_t* __restrict__ y0, const uint16_t* __restrict_
       o[2 * j] = ld16<BF16>(&al) + ld16<BF16>(&cl) * s_scale[c8 * 8 + 2 * j];
       o[2 * j + 1] = ld16<BF16>(&ah) + ld16<BF16>(&ch) * s_scale[c8 * 8 + 2 * j + 1];
     }
-    uint4 u;
-    u.x = pack16x2<BF16>(o[0], o[1]); u.y = pack16x2<BF16>(o[2], o[3]);
-    u.z = pack16x2<BF16>(o[4], o[5]); u.w = pack16x2<BF16>(o[6], o[7]);
-    *reinterpret_cast<uint4*>(y + off) = u;
+    *reinterpret_cast<uint4*>(y + off) = pack8<BF16>(o);
   }
-}
-
-inline unsigned grid_cap(int64_t total, int threads = 256) {
-  int64_t g = (total + threads - 1) / threads;
-  const int64_t cap = 132 * 16;
-  return static_cast<unsigned>(g < cap ? (g > 0 ? g : 1) : cap);
 }
 
 }  // namespace iggt
@@ -171,68 +144,75 @@ using namespace iggt;
 
 extern "C" int iggt_layernorm16(const void* x, void* y, int64_t rows, int C, const float* w, const float* b,
                                 float eps, int dtype, iggt_stream_t stream) {
-  if (rows <= 0) return 0;
-  if (!w || !b) return -1;
-  const unsigned grid = static_cast<unsigned>((rows + 7) / 8);
-  cudaStream_t s = (cudaStream_t)stream;
-#define L16(BF, CC) layernorm16_kernel<BF, CC><<<grid, 256, 0, s>>>((const uint16_t*)x, (uint16_t*)y, w, b, eps, rows)
-  if (C == 256) { if (dtype) L16(true, 256); else L16(false, 256); }
-  else if (C == 128) { if (dtype) L16(true, 128); else L16(false, 128); }
-  else if (C == 64) { if (dtype) L16(true, 64); else L16(false, 64); }
-  else return -1;
+  return dispatch_dtype(dtype, [&](auto bf16) {
+    if (rows <= 0) return 0;
+    if (!w || !b) return -1;
+    const unsigned grid = static_cast<unsigned>((rows + 7) / 8);
+    cudaStream_t s = (cudaStream_t)stream;
+#define L16(CC) layernorm16_kernel<bf16, CC><<<grid, 256, 0, s>>>((const uint16_t*)x, (uint16_t*)y, w, b, eps, rows)
+    if (C == 256) L16(256);
+    else if (C == 128) L16(128);
+    else if (C == 64) L16(64);
+    else return -1;
 #undef L16
-  return (int)cudaGetLastError();
+    return (int)cudaGetLastError();
+  });
 }
 
 extern "C" int iggt_col2im_k4s2p1(const void* Y, const float* bias, void* out, int NB, int h, int w, int C,
                                   int dtype, iggt_stream_t stream) {
-  if (NB <= 0 || (C % 8) || !bias) return -1;
-  const int64_t total = static_cast<int64_t>(NB) * 4 * h * w * (C / 8);
-  if (dtype) col2im_k4s2p1_kernel<true><<<grid_cap(total), 256, 0, (cudaStream_t)stream>>>((const uint16_t*)Y, bias, (uint16_t*)out, NB, h, w, C);
-  else col2im_k4s2p1_kernel<false><<<grid_cap(total), 256, 0, (cudaStream_t)stream>>>((const uint16_t*)Y, bias, (uint16_t*)out, NB, h, w, C);
-  return (int)cudaGetLastError();
+  return dispatch_dtype(dtype, [&](auto bf16) {
+    if (NB <= 0 || (C % 8) || !bias) return -1;
+    const int64_t total = static_cast<int64_t>(NB) * 4 * h * w * (C / 8);
+    col2im_k4s2p1_kernel<bf16><<<grid_stride_blocks(total), 256, 0, (cudaStream_t)stream>>>(
+        (const uint16_t*)Y, bias, (uint16_t*)out, NB, h, w, C);
+    return (int)cudaGetLastError();
+  });
 }
 
 extern "C" int iggt_ocab_attention(const void* q, const void* k, const void* v, const float* table, const int* rpi,
                                    void* out, int NB, int h, int w, int dtype, iggt_stream_t stream) {
-  if (NB <= 0 || (h % 8) || (w % 8)) return -1;
-  static DeviceOnce once;
-  if (once.first()) {
-    cudaFuncSetAttribute(ocab_attention_tc_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, OA_SMEM);
-    cudaFuncSetAttribute(ocab_attention_tc_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, OA_SMEM);
-  }
-  const unsigned grid = static_cast<unsigned>(NB) * (h / 8) * (w / 8) * 4;
-  if (dtype) ocab_attention_tc_kernel<true><<<grid, 128, OA_SMEM, (cudaStream_t)stream>>>((const uint16_t*)q, (const uint16_t*)k, (const uint16_t*)v, table, rpi, (uint16_t*)out, h, w);
-  else ocab_attention_tc_kernel<false><<<grid, 128, OA_SMEM, (cudaStream_t)stream>>>((const uint16_t*)q, (const uint16_t*)k, (const uint16_t*)v, table, rpi, (uint16_t*)out, h, w);
-  return (int)cudaGetLastError();
+  return dispatch_dtype(dtype, [&](auto bf16) {
+    if (NB <= 0 || (h % 8) || (w % 8)) return -1;
+    const cudaError_t e = opt_in_smem<ocab_attention_tc_kernel<bf16>>(OA_SMEM);
+    if (e != cudaSuccess) return (int)e;
+    const unsigned grid = static_cast<unsigned>(NB) * (h / 8) * (w / 8) * 4;
+    ocab_attention_tc_kernel<bf16><<<grid, 128, OA_SMEM, (cudaStream_t)stream>>>(
+        (const uint16_t*)q, (const uint16_t*)k, (const uint16_t*)v, table, rpi, (uint16_t*)out, h, w);
+    return (int)cudaGetLastError();
+  });
 }
 
 extern "C" int iggt_window_attention(const void* qkv, void* out, int NB, int h, int w, int dtype,
                                      iggt_stream_t stream) {
-  if (NB <= 0 || (h % 8) || (w % 8)) return -1;
-  const unsigned grid = static_cast<unsigned>(NB) * (h / 8) * (w / 8) * 4;
-  if (dtype) window_attention_tc_kernel<true><<<grid, 128, 0, (cudaStream_t)stream>>>((const uint16_t*)qkv, (uint16_t*)out, h, w);
-  else window_attention_tc_kernel<false><<<grid, 128, 0, (cudaStream_t)stream>>>((const uint16_t*)qkv, (uint16_t*)out, h, w);
-  return (int)cudaGetLastError();
+  return dispatch_dtype(dtype, [&](auto bf16) {
+    if (NB <= 0 || (h % 8) || (w % 8)) return -1;
+    const unsigned grid = static_cast<unsigned>(NB) * (h / 8) * (w / 8) * 4;
+    window_attention_tc_kernel<bf16><<<grid, 128, 0, (cudaStream_t)stream>>>((const uint16_t*)qkv, (uint16_t*)out, h, w);
+    return (int)cudaGetLastError();
+  });
 }
 
 extern "C" int iggt_channel_mean(const void* x, float* mean, int NB, int64_t hw, int C, int dtype,
                                  iggt_stream_t stream) {
-  if (NB <= 0 || C <= 0 || C > 256 || (256 % C)) return -1;
-  cudaError_t e = cudaMemsetAsync(mean, 0, sizeof(float) * NB * C, (cudaStream_t)stream);
-  if (e != cudaSuccess) return (int)e;
-  dim3 grid(static_cast<unsigned>(hw / 64 > 0 ? (hw / 64 < 296 ? hw / 64 : 296) : 1), NB);
-  if (dtype) channel_mean_kernel<true><<<grid, 256, 0, (cudaStream_t)stream>>>((const uint16_t*)x, mean, hw, C, 1.0f / hw);
-  else channel_mean_kernel<false><<<grid, 256, 0, (cudaStream_t)stream>>>((const uint16_t*)x, mean, hw, C, 1.0f / hw);
-  return (int)cudaGetLastError();
+  return dispatch_dtype(dtype, [&](auto bf16) {
+    if (NB <= 0 || C <= 0 || C > 256 || (256 % C)) return -1;
+    cudaError_t e = cudaMemsetAsync(mean, 0, sizeof(float) * NB * C, (cudaStream_t)stream);
+    if (e != cudaSuccess) return (int)e;
+    dim3 grid(static_cast<unsigned>(hw / 64 > 0 ? (hw / 64 < 296 ? hw / 64 : 296) : 1), NB);
+    channel_mean_kernel<bf16><<<grid, 256, 0, (cudaStream_t)stream>>>((const uint16_t*)x, mean, hw, C, 1.0f / hw);
+    return (int)cudaGetLastError();
+  });
 }
 
 extern "C" int iggt_se_scale_add(const void* y0, const void* cx, const float* mean, const float* w1, const float* b1,
                                  const float* w2, const float* b2, void* y, int NB, int64_t hw, int C, int R,
                                  float alpha, int dtype, iggt_stream_t stream) {
-  if (NB <= 0 || C > 256 || (C % 8) || R > 16) return -1;
-  dim3 grid(grid_cap(hw * (C / 8)) / 2 + 1, NB);
-  if (dtype) se_scale_add_kernel<true><<<grid, 256, 0, (cudaStream_t)stream>>>((const uint16_t*)y0, (const uint16_t*)cx, mean, w1, b1, w2, b2, (uint16_t*)y, hw, C, R, alpha);
-  else se_scale_add_kernel<false><<<grid, 256, 0, (cudaStream_t)stream>>>((const uint16_t*)y0, (const uint16_t*)cx, mean, w1, b1, w2, b2, (uint16_t*)y, hw, C, R, alpha);
-  return (int)cudaGetLastError();
+  return dispatch_dtype(dtype, [&](auto bf16) {
+    if (NB <= 0 || C > 256 || (C % 8) || R > 16) return -1;
+    dim3 grid(grid_stride_blocks(hw * (C / 8)) / 2 + 1, NB);
+    se_scale_add_kernel<bf16><<<grid, 256, 0, (cudaStream_t)stream>>>(
+        (const uint16_t*)y0, (const uint16_t*)cx, mean, w1, b1, w2, b2, (uint16_t*)y, hw, C, R, alpha);
+    return (int)cudaGetLastError();
+  });
 }

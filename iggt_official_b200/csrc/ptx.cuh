@@ -281,6 +281,51 @@ __device__ __forceinline__ uint32_t pack16x2(float a, float b) {
   if constexpr (BF16) return pack_bf16x2(a, b);
   else return pack_f16x2(a, b);
 }
+// one 16-bit element <-> fp32 (round to nearest even)
+template <bool BF16>
+__device__ __forceinline__ float ld16(const uint16_t* p) {
+  if constexpr (BF16) return __uint_as_float(static_cast<uint32_t>(*p) << 16);
+  else return __half2float(__ushort_as_half(*p));
+}
+template <bool BF16>
+__device__ __forceinline__ uint16_t st16(float v) {
+  if constexpr (BF16) return __bfloat16_as_ushort(__float2bfloat16_rn(v));
+  else return __half_as_ushort(__float2half_rn(v));
+}
+// two / eight packed 16-bit elements <-> fp32 (one 32-bit word, one 16-byte vector)
+template <bool BF16>
+__device__ __forceinline__ float2 cvt16x2(uint32_t u) {
+  if constexpr (BF16) return make_float2(__uint_as_float(u << 16), __uint_as_float(u & 0xFFFF0000u));
+  else return __half22float2(*reinterpret_cast<const __half2*>(&u));
+}
+template <bool BF16>
+__device__ __forceinline__ void unpack8(const uint4& u, float (&f)[8]) {
+  const uint32_t w[4] = {u.x, u.y, u.z, u.w};
+#pragma unroll
+  for (int j = 0; j < 4; ++j) {
+    if constexpr (BF16) {
+      f[2 * j] = __uint_as_float(w[j] << 16);
+      f[2 * j + 1] = __uint_as_float(w[j] & 0xFFFF0000u);
+    } else {
+      const __half2 h = *reinterpret_cast<const __half2*>(&w[j]);
+      f[2 * j] = __low2float(h);
+      f[2 * j + 1] = __high2float(h);
+    }
+  }
+}
+template <bool BF16>
+__device__ __forceinline__ uint4 pack8(const float (&f)[8]) {
+  uint4 u;
+  u.x = pack16x2<BF16>(f[0], f[1]); u.y = pack16x2<BF16>(f[2], f[3]);
+  u.z = pack16x2<BF16>(f[4], f[5]); u.w = pack16x2<BF16>(f[6], f[7]);
+  return u;
+}
+// butterfly sum over the 32 lanes of a warp: every lane gets the total
+__device__ __forceinline__ float warp_sum(float v) {
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+  return v;
+}
 // ReLU that keeps a NaN (torch.relu's behaviour; fmaxf would return 0 and hide an overflowed head activation)
 __device__ __forceinline__ float relu_nan(float x) {
   float y;

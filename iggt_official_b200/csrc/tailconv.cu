@@ -226,15 +226,11 @@ tailconv_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
 
 template <bool BF16>
 int launch_tailconv(const CUtensorMap& tA, const CUtensorMap& tB, const TailConvParams& p, cudaStream_t stream) {
-  auto kern = tailconv_kernel<BF16>;
-  static DeviceOnce once;
-  if (once.first()) {
-    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, TC_SMEM);
-    if (e != cudaSuccess) { once.reset_current(); return (int)e; }
-  }
+  const cudaError_t e = opt_in_smem<tailconv_kernel<BF16>>(TC_SMEM);
+  if (e != cudaSuccess) return (int)e;
   const int sms = device_sm_count();
   const int grid = p.total_tiles < sms ? p.total_tiles : sms;
-  return (int)launch_pdl(kern, dim3(grid), dim3(TC_THREADS), TC_SMEM, stream, tA, tB, p);
+  return (int)launch_pdl(tailconv_kernel<BF16>, dim3(grid), dim3(TC_THREADS), TC_SMEM, stream, tA, tB, p);
 }
 
 }  // namespace iggt
@@ -244,29 +240,29 @@ using namespace iggt;
 extern "C" int iggt_dpt_tail_fused(const void* x, const void* Wp, const float* bias, const float* w2, const float* b2,
                                    float* out_main, float* out_conf, void* out16, int NB, int H, int W, int OC, int mode,
                                    int dtype, iggt_stream_t stream) {
-  if (!x || !Wp || NB <= 0 || H <= 0 || W <= 0) return -1;
-  if (dtype != 0 && dtype != 1) return -3;
-  if (w2) {
-    if (!b2 || !out_main || (OC != 2 && OC != 4 && OC != 8) || mode < 0 || mode > 2) return -1;
-    if (mode != 2 && !out_conf) return -1;
-  } else if (!out16) {
-    return -1;
-  }
-  const TmDtype dt = dtype ? TM_BF16 : TM_F16;
-  CUtensorMap tA, tB;
-  {
-    uint64_t dims[4] = {(uint64_t)TC_CIN, (uint64_t)W, (uint64_t)H, (uint64_t)NB};
-    uint64_t str[3] = {(uint64_t)TC_CIN * 2, (uint64_t)W * TC_CIN * 2, (uint64_t)H * W * TC_CIN * 2};
-    uint32_t box[4] = {64, TC_TW, TC_BOX_ROWS, 1};
-    if (make_tmap(&tA, dt, 4, x, dims, str, box)) return -4;
-  }
-  if (make_tmap_2d(&tB, dt, Wp, (uint64_t)TC_N, (uint64_t)9 * TC_CIN, (uint64_t)9 * TC_CIN, 64, TC_N)) return -4;
-  TailConvParams p;
-  p.NB = NB; p.H = H; p.W = W;
-  p.tiles_x = (W + TC_TW - 1) / TC_TW;
-  p.tiles_y = (H + TC_TH - 1) / TC_TH;
-  p.total_tiles = NB * p.tiles_x * p.tiles_y;
-  p.bias = bias; p.w2 = w2; p.b2 = b2; p.OC = OC; p.mode = mode;
-  p.out_main = out_main; p.out_conf = out_conf; p.out16 = out16;
-  return dtype ? launch_tailconv<true>(tA, tB, p, (cudaStream_t)stream) : launch_tailconv<false>(tA, tB, p, (cudaStream_t)stream);
+  return dispatch_dtype(dtype, [&](auto bf16) {
+    if (!x || !Wp || NB <= 0 || H <= 0 || W <= 0) return -1;
+    if (w2) {
+      if (!b2 || !out_main || (OC != 2 && OC != 4 && OC != 8) || mode < 0 || mode > 2) return -1;
+      if (mode != 2 && !out_conf) return -1;
+    } else if (!out16) {
+      return -1;
+    }
+    CUtensorMap tA, tB;
+    {
+      uint64_t dims[4] = {(uint64_t)TC_CIN, (uint64_t)W, (uint64_t)H, (uint64_t)NB};
+      uint64_t str[3] = {(uint64_t)TC_CIN * 2, (uint64_t)W * TC_CIN * 2, (uint64_t)H * W * TC_CIN * 2};
+      uint32_t box[4] = {64, TC_TW, TC_BOX_ROWS, 1};
+      if (make_tmap(&tA, tm16(bf16), 4, x, dims, str, box)) return -4;
+    }
+    if (make_tmap_2d(&tB, tm16(bf16), Wp, (uint64_t)TC_N, (uint64_t)9 * TC_CIN, (uint64_t)9 * TC_CIN, 64, TC_N)) return -4;
+    TailConvParams p;
+    p.NB = NB; p.H = H; p.W = W;
+    p.tiles_x = (W + TC_TW - 1) / TC_TW;
+    p.tiles_y = (H + TC_TH - 1) / TC_TH;
+    p.total_tiles = NB * p.tiles_x * p.tiles_y;
+    p.bias = bias; p.w2 = w2; p.b2 = b2; p.OC = OC; p.mode = mode;
+    p.out_main = out_main; p.out_conf = out_conf; p.out16 = out16;
+    return launch_tailconv<bf16>(tA, tB, p, (cudaStream_t)stream);
+  });
 }

@@ -29,6 +29,8 @@ inline EncodeTiledFn get_encode_fn() {
 }
 
 enum TmDtype { TM_F16 = 0, TM_BF16 = 1, TM_F32 = 2, TM_U8 = 3 };
+// element type of a 16-bit operand (the launchers' dtype, resolved by dispatch_dtype)
+constexpr TmDtype tm16(bool bf16) { return bf16 ? TM_BF16 : TM_F16; }
 
 // Generic rank<=4 tiled map. dims[0] is the contiguous dimension; strides_bytes[i] is the pitch of
 // dimension i+1 (rank-1 entries). 128-byte swizzle; out-of-bounds elements read as zero.

@@ -8,29 +8,11 @@
 //   track_input          flow embedding + concatenation + positional / reference tokens + LayerNorm(388) in one pass
 //                        (base_track_predictor.py:139-165 + blocks.py:103-104)
 //   layernorm_rows       LayerNorm over any width <= 2048 of fp32 rows, fp32 and / or 16-bit result
-#include <cuda_bf16.h>
-#include <cuda_fp16.h>
-#include <cuda_runtime.h>
-#include <stdint.h>
+#include "ptx.cuh"
+#include "launch.cuh"
 #include "../../include/iggt_b200.h"
 
 namespace iggt {
-
-template <bool BF16>
-__device__ __forceinline__ float ld16(const uint16_t* p) {
-  if constexpr (BF16) return __uint_as_float(static_cast<uint32_t>(*p) << 16);
-  else return __half2float(__ushort_as_half(*p));
-}
-template <bool BF16>
-__device__ __forceinline__ uint16_t st16(float v) {
-  if constexpr (BF16) return __bfloat16_as_ushort(__float2bfloat16_rn(v));
-  else return __half_as_ushort(__float2half_rn(v));
-}
-__device__ __forceinline__ float warp_sum(float v) {
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-  return v;
-}
 
 // [NB, H, W, C] -> [NB, H/2, W/2, C] (floor), fp32 mean of the 2x2 window, one thread per 2 channels
 template <bool BF16>
@@ -232,70 +214,69 @@ layernorm_rows_kernel(const float* __restrict__ x, int64_t ldx, int C, const flo
   }
 }
 
-inline unsigned cap_grid(int64_t work, int per_block) {
-  const int64_t g = (work + per_block - 1) / per_block;
-  return static_cast<unsigned>(g < 1 ? 1 : (g > 132 * 16 ? 132 * 16 : g));
-}
-
 }  // namespace iggt
 
 using namespace iggt;
 
 extern "C" int iggt_avgpool2_nhwc(const void* x, void* y, int NB, int H, int W, int C, int dtype, iggt_stream_t stream) {
-  if (!x || !y || NB <= 0 || H < 2 || W < 2 || C <= 0 || (C & 1)) return -1;
-  const int64_t total = static_cast<int64_t>(NB) * (H / 2) * (W / 2) * (C / 2);
-  cudaStream_t s = (cudaStream_t)stream;
-  if (dtype) avgpool2_kernel<true><<<cap_grid(total, 256), 256, 0, s>>>((const uint16_t*)x, (uint16_t*)y, NB, H, W, C);
-  else avgpool2_kernel<false><<<cap_grid(total, 256), 256, 0, s>>>((const uint16_t*)x, (uint16_t*)y, NB, H, W, C);
-  return (int)cudaGetLastError();
+  return dispatch_dtype(dtype, [&](auto bf16) {
+    if (!x || !y || NB <= 0 || H < 2 || W < 2 || C <= 0 || (C & 1)) return -1;
+    const int64_t total = static_cast<int64_t>(NB) * (H / 2) * (W / 2) * (C / 2);
+    avgpool2_kernel<bf16><<<grid_stride_blocks(total), 256, 0, (cudaStream_t)stream>>>((const uint16_t*)x, (uint16_t*)y,
+                                                                                       NB, H, W, C);
+    return (int)cudaGetLastError();
+  });
 }
 
 extern "C" int iggt_sample_bilinear_nhwc(const void* x, const float* coords, float* out, int NB, int R, int H, int W, int C,
                                          int dtype, iggt_stream_t stream) {
-  if (!x || !coords || !out || NB <= 0 || R <= 0 || H <= 0 || W <= 0 || C <= 0) return -1;
-  const unsigned grid = static_cast<unsigned>((static_cast<int64_t>(NB) * R + 7) / 8);
-  cudaStream_t s = (cudaStream_t)stream;
-  if (dtype) sample_bilinear_kernel<true><<<grid, 256, 0, s>>>((const uint16_t*)x, coords, out, NB, R, H, W, C);
-  else sample_bilinear_kernel<false><<<grid, 256, 0, s>>>((const uint16_t*)x, coords, out, NB, R, H, W, C);
-  return (int)cudaGetLastError();
+  return dispatch_dtype(dtype, [&](auto bf16) {
+    if (!x || !coords || !out || NB <= 0 || R <= 0 || H <= 0 || W <= 0 || C <= 0) return -1;
+    const unsigned grid = static_cast<unsigned>((static_cast<int64_t>(NB) * R + 7) / 8);
+    sample_bilinear_kernel<bf16><<<grid, 256, 0, (cudaStream_t)stream>>>((const uint16_t*)x, coords, out, NB, R, H, W, C);
+    return (int)cudaGetLastError();
+  });
 }
 
 extern "C" int iggt_corr_sample(const void* const* levels, const int* Hs, const int* Ws, const float* targets,
                                 const float* coords, void* out, int B, int N, int S, int ldo, int dtype,
                                 iggt_stream_t stream) {
-  if (!levels || !Hs || !Ws || !targets || !coords || !out || B <= 0 || N <= 0 || S <= 0) return -1;
-  if (ldo < CORR_LEVELS * CORR_WIN * CORR_WIN) return -2;
-  CorrParams p;
-  for (int l = 0; l < CORR_LEVELS; ++l) {
-    if (!levels[l] || Hs[l] <= 0 || Ws[l] <= 0) return -1;
-    p.level[l] = static_cast<const uint16_t*>(levels[l]); p.H[l] = Hs[l]; p.W[l] = Ws[l];
-  }
-  p.targets = targets; p.coords = coords; p.out = out;
-  p.rows = B * N * S; p.N = N; p.S = S; p.ldo = ldo;
-  const unsigned grid = static_cast<unsigned>((static_cast<int64_t>(p.rows) * CORR_LEVELS + 7) / 8);
-  if (dtype) corr_sample_kernel<true><<<grid, 256, 0, (cudaStream_t)stream>>>(p);
-  else corr_sample_kernel<false><<<grid, 256, 0, (cudaStream_t)stream>>>(p);
-  return (int)cudaGetLastError();
+  return dispatch_dtype(dtype, [&](auto bf16) {
+    if (!levels || !Hs || !Ws || !targets || !coords || !out || B <= 0 || N <= 0 || S <= 0) return -1;
+    if (ldo < CORR_LEVELS * CORR_WIN * CORR_WIN) return -2;
+    CorrParams p;
+    for (int l = 0; l < CORR_LEVELS; ++l) {
+      if (!levels[l] || Hs[l] <= 0 || Ws[l] <= 0) return -1;
+      p.level[l] = static_cast<const uint16_t*>(levels[l]); p.H[l] = Hs[l]; p.W[l] = Ws[l];
+    }
+    p.targets = targets; p.coords = coords; p.out = out;
+    p.rows = B * N * S; p.N = N; p.S = S; p.ldo = ldo;
+    const unsigned grid = static_cast<unsigned>((static_cast<int64_t>(p.rows) * CORR_LEVELS + 7) / 8);
+    corr_sample_kernel<bf16><<<grid, 256, 0, (cudaStream_t)stream>>>(p);
+    return (int)cudaGetLastError();
+  });
 }
 
 extern "C" int iggt_track_input(const float* coords, const float* fcorr, const float* tfeat, const float* pos,
                                 const float* ref_tok, const float* ln_w, const float* ln_b, void* out, float* raw,
                                 int rows, int S, int ldo, float eps, int dtype, iggt_stream_t stream) {
-  if (!coords || !fcorr || !tfeat || !pos || !ref_tok || !ln_w || !ln_b || !out || rows <= 0 || S <= 0) return -1;
-  if (ldo < 388 || ldo > 416) return -2;
-  const unsigned grid = static_cast<unsigned>((rows + 7) / 8);
-  cudaStream_t s = (cudaStream_t)stream;
-  if (dtype) track_input_kernel<true><<<grid, 256, 0, s>>>(coords, fcorr, tfeat, pos, ref_tok, ln_w, ln_b, (uint16_t*)out, raw, rows, S, ldo, eps);
-  else track_input_kernel<false><<<grid, 256, 0, s>>>(coords, fcorr, tfeat, pos, ref_tok, ln_w, ln_b, (uint16_t*)out, raw, rows, S, ldo, eps);
-  return (int)cudaGetLastError();
+  return dispatch_dtype(dtype, [&](auto bf16) {
+    if (!coords || !fcorr || !tfeat || !pos || !ref_tok || !ln_w || !ln_b || !out || rows <= 0 || S <= 0) return -1;
+    if (ldo < 388 || ldo > 416) return -2;
+    const unsigned grid = static_cast<unsigned>((rows + 7) / 8);
+    track_input_kernel<bf16><<<grid, 256, 0, (cudaStream_t)stream>>>(coords, fcorr, tfeat, pos, ref_tok, ln_w, ln_b,
+                                                                     (uint16_t*)out, raw, rows, S, ldo, eps);
+    return (int)cudaGetLastError();
+  });
 }
 
 extern "C" int iggt_layernorm_rows(const float* x, int64_t ldx, int C, const float* w, const float* b, float eps,
                                    int64_t rows, float* y32, void* y16, int ld16, int dtype, iggt_stream_t stream) {
-  if (!x || !w || !b || C <= 0 || C > 2048 || rows <= 0 || (!y32 && !y16) || (y16 && ld16 < C)) return -1;
-  const unsigned grid = static_cast<unsigned>((rows + 7) / 8);
-  cudaStream_t s = (cudaStream_t)stream;
-  if (dtype) layernorm_rows_kernel<true><<<grid, 256, 0, s>>>(x, ldx, C, w, b, eps, rows, y32, (uint16_t*)y16, ld16);
-  else layernorm_rows_kernel<false><<<grid, 256, 0, s>>>(x, ldx, C, w, b, eps, rows, y32, (uint16_t*)y16, ld16);
-  return (int)cudaGetLastError();
+  return dispatch_dtype(dtype, [&](auto bf16) {
+    if (!x || !w || !b || C <= 0 || C > 2048 || rows <= 0 || (!y32 && !y16) || (y16 && ld16 < C)) return -1;
+    const unsigned grid = static_cast<unsigned>((rows + 7) / 8);
+    layernorm_rows_kernel<bf16><<<grid, 256, 0, (cudaStream_t)stream>>>(x, ldx, C, w, b, eps, rows, y32, (uint16_t*)y16,
+                                                                        ld16);
+    return (int)cudaGetLastError();
+  });
 }

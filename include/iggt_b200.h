@@ -8,7 +8,8 @@
  * >0 = cudaError_t).  Each entry cites the reference call site it replaces.  All pointers are device
  * pointers unless stated otherwise; all launches are asynchronous on `stream`.
  *
- * dtype: 0 = fp16, 1 = bf16 (16-bit activations / weights; accumulation is always fp32).
+ * dtype: 0 = fp16, 1 = bf16 (16-bit activations / weights; accumulation is always fp32).  Any other dtype code
+ * returns -3 before any work: before the other argument checks and before any CUDA call.
  */
 #ifndef IGGT_B200_H_
 #define IGGT_B200_H_
@@ -21,7 +22,7 @@ extern "C" {
 
 typedef void* iggt_stream_t; /* cudaStream_t */
 
-/* Library / device probe. Returns 0 and fills sm (e.g. 100) and num_sms, or >0 cudaError_t. */
+/* Library / device probe. Returns 0 and fills sm (e.g. 90) and num_sms, or >0 cudaError_t. */
 int iggt_device_info(int* sm, int* num_sms);
 const char* iggt_version(void);
 
@@ -103,8 +104,9 @@ int iggt_attention_schedule_splits(int num_seq, int Lq, int Lk, int H, int split
 
 /* LayerNorm over C (1024 or 2048) fp32 features, one warp per row.  Output row g*out_rows_per_group +
  * out_off + i  <-  input row g*rows_in + in_off + i, for g < groups, i < rows_out.  w/b may be NULL.
- * out_kind: 0 fp16, 1 bf16, 2 fp32.  Replaces nn.LayerNorm at iggt/layers/block.py:50,66,
- * iggt/layers/vision_transformer.py:274, iggt/heads/dpt_head.py:234. */
+ * out_kind: 0 fp16, 1 bf16, 2 fp32; any other code returns -3 before any work, as an invalid dtype does.
+ * Replaces nn.LayerNorm at iggt/layers/block.py:50,66, iggt/layers/vision_transformer.py:274,
+ * iggt/heads/dpt_head.py:234. */
 int iggt_layernorm(const float* x, int64_t ldx, void* y, int64_t ldy, int C, const float* w,
                    const float* b, float eps, int64_t groups, int rows_out, int rows_in, int in_off,
                    int out_rows_per_group, int out_off, int out_kind, iggt_stream_t stream);
