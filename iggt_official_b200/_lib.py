@@ -50,6 +50,7 @@ SIGNATURES = {
     "iggt_skinny_gemm": [c_void_p, c_int64, c_void_p, c_int64, c_void_p, c_void_p, c_void_p, c_int64, c_void_p,
                          c_int64, c_int, c_int, c_int, c_int, c_int, c_void_p],
     "iggt_small_attention": [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_float, c_void_p],
+    "iggt_token_attention": [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_float, c_void_p],
     "iggt_camera_head_workspace": [c_int],
     "iggt_camera_head": [c_void_p, c_void_p, c_int64, c_void_p, c_void_p, c_int64, c_int, c_int, c_int, c_int, c_void_p],
     "iggt_layernorm16": [c_void_p, c_void_p, c_int64, c_int, c_void_p, c_void_p, c_float, c_int, c_void_p],

@@ -255,6 +255,122 @@ small_attention_kernel(const float* __restrict__ qkv, float* __restrict__ out, i
   }
 }
 
+// softmax(q k^T / sqrt(d)) v over any number of keys (camera tokens of scenes with more views than small_attention's
+// shared memory holds), fp32 on the CUDA cores.  Same layout as small_attention.  One CTA per (b, head, block of TA_QB
+// query rows); the keys and values of the scene go through shared memory in tiles of TA_KT rows, in key order, so the
+// shared memory is a constant independent of N.  Warp w owns query rows 4w..4w+3 of the block; lane l scores keys l and
+// l + 32 of the tile (a sequential fmaf chain over d, then * scale, as small_attention) and owns output columns
+// l + 32 i.  Online softmax per row: a running max m and sum l; when a tile raises the max, acc and l are rescaled by
+// expf(m_old - m_new) (a factor of exactly 1 otherwise), p = expf(s - m_new), the tile's p are summed by the lanes
+// (p0 + p1, then a butterfly) and added to l, and acc takes the tile's keys in key order with fmaf.  out = acc * (1/l).
+// No atomics, a fixed tile order: repeated calls are bit-identical.
+constexpr int TA_KT = 64;          // keys per tile
+constexpr int TA_QB = 16;          // query rows per CTA (4 warps x 4 rows)
+constexpr int TA_DMAX = 128;
+constexpr int TA_LD_MAX = TA_DMAX + 4;   // row pitch d + 4: lanes reading float4s of 8 consecutive rows hit distinct banks
+constexpr int TA_SMEM = (2 * TA_KT + TA_QB) * TA_LD_MAX * static_cast<int>(sizeof(float));   // 76032 B
+template <int NC>                  // NC = d / 32 output columns per lane
+__global__ void __launch_bounds__(128, 2)
+token_attention_kernel(const float* __restrict__ qkv, float* __restrict__ out, int N, int H, float scale) {
+  constexpr int d = NC * 32, ld = d + 4;
+  extern __shared__ __align__(16) float ta_smem[];
+  float* sk = ta_smem;                      // [TA_KT][ld]
+  float* sv = sk + TA_KT * ld;              // [TA_KT][ld]
+  float* sq = sv + TA_KT * ld;              // [TA_QB][ld]
+  const int b = blockIdx.x / H, hh = blockIdx.x % H;
+  const int q0 = blockIdx.y * TA_QB;
+  const int64_t C = static_cast<int64_t>(H) * d;
+  const float* base = qkv + static_cast<int64_t>(b) * N * 3 * C + hh * d;     // q of row 0 of scene b, head hh
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  constexpr int V4 = d / 4;                 // float4 per row
+  for (int i = threadIdx.x; i < TA_QB * V4; i += blockDim.x) {
+    const int r = i / V4, c4 = i - r * V4;
+    float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
+    if (q0 + r < N) v = __ldg(reinterpret_cast<const float4*>(base + static_cast<int64_t>(q0 + r) * 3 * C) + c4);
+    *reinterpret_cast<float4*>(sq + r * ld + c4 * 4) = v;
+  }
+  float m[4], l[4], acc[4][NC];
+#pragma unroll
+  for (int r = 0; r < 4; ++r) {
+    m[r] = -INFINITY; l[r] = 0.f;
+#pragma unroll
+    for (int i = 0; i < NC; ++i) acc[r][i] = 0.f;
+  }
+  const int rows = min(4, max(0, N - q0 - warp * 4));          // valid query rows of this warp
+  for (int t0 = 0; t0 < N; t0 += TA_KT) {
+    const int nk = min(TA_KT, N - t0);
+    __syncthreads();                        // the previous tile is consumed (and the q rows are stored)
+    for (int i = threadIdx.x; i < TA_KT * V4; i += blockDim.x) {
+      const int r = i / V4, c4 = i - r * V4;
+      float4 kv = make_float4(0.f, 0.f, 0.f, 0.f), vv = kv;
+      if (r < nk) {
+        const float* row = base + static_cast<int64_t>(t0 + r) * 3 * C;
+        kv = __ldg(reinterpret_cast<const float4*>(row + C) + c4);
+        vv = __ldg(reinterpret_cast<const float4*>(row + 2 * C) + c4);
+      }
+      *reinterpret_cast<float4*>(sk + r * ld + c4 * 4) = kv;
+      *reinterpret_cast<float4*>(sv + r * ld + c4 * 4) = vv;
+    }
+    __syncthreads();
+    if (rows == 0) continue;
+    float s[4][2];
+#pragma unroll
+    for (int r = 0; r < 4; ++r) s[r][0] = s[r][1] = 0.f;
+    const float* k0 = sk + lane * ld;
+    const float* k1 = sk + (lane + 32) * ld;
+    const float* qw = sq + warp * 4 * ld;
+#pragma unroll 4
+    for (int c = 0; c < d; c += 4) {
+      const float4 a = *reinterpret_cast<const float4*>(k0 + c);
+      const float4 e = *reinterpret_cast<const float4*>(k1 + c);
+#pragma unroll
+      for (int r = 0; r < 4; ++r) {
+        const float4 q = *reinterpret_cast<const float4*>(qw + r * ld + c);
+        s[r][0] = fmaf(q.x, a.x, s[r][0]); s[r][0] = fmaf(q.y, a.y, s[r][0]);
+        s[r][0] = fmaf(q.z, a.z, s[r][0]); s[r][0] = fmaf(q.w, a.w, s[r][0]);
+        s[r][1] = fmaf(q.x, e.x, s[r][1]); s[r][1] = fmaf(q.y, e.y, s[r][1]);
+        s[r][1] = fmaf(q.z, e.z, s[r][1]); s[r][1] = fmaf(q.w, e.w, s[r][1]);
+      }
+    }
+    float p[4][2];
+#pragma unroll
+    for (int r = 0; r < 4; ++r) {
+      const float s0 = lane < nk ? s[r][0] * scale : -INFINITY;
+      const float s1 = lane + 32 < nk ? s[r][1] * scale : -INFINITY;
+      float mt = fmaxf(s0, s1);
+#pragma unroll
+      for (int o = 16; o > 0; o >>= 1) mt = fmaxf(mt, __shfl_xor_sync(0xffffffffu, mt, o));
+      const float mn = fmaxf(m[r], mt);
+      const float alpha = expf(m[r] - mn);  // 0 at the first tile (m = -inf), 1 when the max did not grow
+      m[r] = mn;
+      p[r][0] = expf(s0 - mn);
+      p[r][1] = expf(s1 - mn);
+      l[r] = __fmaf_rn(l[r], alpha, warp_sum(p[r][0] + p[r][1]));
+#pragma unroll
+      for (int i = 0; i < NC; ++i) acc[r][i] *= alpha;
+    }
+    for (int j = 0; j < nk; ++j) {
+      float vj[NC];
+#pragma unroll
+      for (int i = 0; i < NC; ++i) vj[i] = sv[j * ld + lane + 32 * i];
+#pragma unroll
+      for (int r = 0; r < 4; ++r) {
+        const float pj = __shfl_sync(0xffffffffu, j < 32 ? p[r][0] : p[r][1], j & 31);
+#pragma unroll
+        for (int i = 0; i < NC; ++i) acc[r][i] = fmaf(pj, vj[i], acc[r][i]);
+      }
+    }
+  }
+#pragma unroll
+  for (int r = 0; r < 4; ++r) {
+    if (r >= rows) break;
+    const float inv = 1.0f / l[r];
+    float* o = out + (static_cast<int64_t>(b) * N + q0 + warp * 4 + r) * C + hh * d;
+#pragma unroll
+    for (int i = 0; i < NC; ++i) o[lane + 32 * i] = acc[r][i] * inv;
+  }
+}
+
 }  // namespace iggt
 
 using namespace iggt;
@@ -327,5 +443,29 @@ extern "C" int iggt_small_attention(const float* qkv, float* out, int B, int N, 
   const cudaError_t e = opt_in_smem<small_attention_kernel>(200 * 1024);
   if (e != cudaSuccess) return (int)e;
   small_attention_kernel<<<B * H, 128, smem, (cudaStream_t)stream>>>(qkv, out, N, H, d, scale);
+  return (int)cudaGetLastError();
+}
+
+extern "C" int iggt_token_attention(const float* qkv, float* out, int B, int N, int H, int d, float scale,
+                                    iggt_stream_t stream) {
+  if (B <= 0 || N <= 0 || H <= 0 || d <= 0 || d > TA_DMAX || (d % 32)) return -1;
+  const int64_t qblocks = (static_cast<int64_t>(N) + TA_QB - 1) / TA_QB;
+  if (qblocks > 65535 || static_cast<int64_t>(B) * H > 0x7fffffff) return -1;
+  // the largest element index, (B*N) * (3*H*d), must fit int64: check in steps that cannot overflow themselves
+  const int64_t rows = static_cast<int64_t>(B) * N, width = 3 * static_cast<int64_t>(H) * d;
+  if (rows > INT64_MAX / width) return -1;
+  if (reinterpret_cast<uintptr_t>(qkv) % 16) return -1;           // float4 loads of the q, k and v rows
+  void (*kern)(const float*, float*, int, int, float);
+  switch (d / 32) {
+    case 1: kern = token_attention_kernel<1>; break;
+    case 2: kern = token_attention_kernel<2>; break;
+    case 3: kern = token_attention_kernel<3>; break;
+    default: kern = token_attention_kernel<4>; break;
+  }
+  const cudaError_t e = opt_in_smem<token_attention_kernel<1>, token_attention_kernel<2>, token_attention_kernel<3>,
+                                    token_attention_kernel<4>>(TA_SMEM);
+  if (e != cudaSuccess) return (int)e;
+  const dim3 grid(static_cast<unsigned>(B * H), static_cast<unsigned>(qblocks));
+  kern<<<grid, 128, TA_SMEM, (cudaStream_t)stream>>>(qkv, out, N, H, scale);
   return (int)cudaGetLastError();
 }

@@ -6,7 +6,9 @@ weights, fp32 accumulate).  For B*S <= 16 the whole head - 4 iterations x (embed
 persistent launch (`iggt_camera_head`, csrc/camera.cu: the producer warp streams weights across phase boundaries, a
 device-wide barrier separates the ~27 phases of an iteration).  Scenes of more than 16 views and devices with fewer
 than 128 SMs (an H100 PCIe, a MIG slice) run layer by layer: `iggt_skinny_gemm`, `iggt_small_attention`,
-`iggt_layernorm`, with the AdaLN modulate in torch arithmetic.
+`iggt_layernorm`, with the AdaLN modulate in torch arithmetic.  Scenes with more views than `iggt_small_attention` holds
+in shared memory (197 and up at head dim 128) take `iggt_token_attention`, which streams the keys, so the view count
+is bounded by device memory only.
 """
 import ctypes
 from typing import List
@@ -114,7 +116,9 @@ class CameraHead(Node):
         h = torch.empty_like(x)
         ops.layernorm(x, w["n1w"], w["n1b"], 1e-5, h)
         qkv = self._rows(ops.skinny_gemm, h, w["qkv_w"], w["qkv_b"])
-        o = ops.small_attention(qkv, B, S, HEADS, DIM // HEADS)
+        # scenes with more views than small_attention holds in shared memory stream their keys (token_attention)
+        attend = ops.small_attention if ops._small_attention_fits(S, DIM // HEADS) else ops.token_attention
+        o = attend(qkv, B, S, HEADS, DIM // HEADS)
         x = self._rows(ops.skinny_gemm, o, w["proj_w"], w["proj_b"], gamma=w["ls1"], resid=x)
         ops.layernorm(x, w["n2w"], w["n2b"], 1e-5, h)
         f = self._rows(ops.skinny_gemm, h, w["fc1_w"], w["fc1_b"], act=1)

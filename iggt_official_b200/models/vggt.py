@@ -15,7 +15,9 @@ Differences from the reference that a caller can observe:
     accumulation whatever the trunk dtype is.  `model.head_dtype = torch.bfloat16` trades 3 mantissa bits for fp32's
     exponent range; `model.check_finite = True` makes forward raise FloatingPointError when an output is not
     finite (e.g. a checkpoint whose head activations exceed fp16's 65504) instead of returning inf / nan.
-  * S > 12 views works (the reference's frame-chunk path raises TypeError, SURVEY F3).
+  * S > 12 views works (the reference's frame-chunk path raises TypeError, SURVEY F3), and any number of views per
+    scene is accepted: the camera head's token attention streams its keys above 196 views, so the view count is
+    bounded by device memory only.
   * `query_points` runs the native track head (heads/track_head.py, reference iggt/models/vggt.py:220-226) and adds
     `track`, `vis`, `conf` to the dictionary exactly like the reference; S > 12 works there too.
 """

@@ -315,12 +315,43 @@ def skinny_gemm(x, w, bias=None, act=0, gamma=None, resid=None, out=None):
     return out
 
 
+def _small_attention_fits(N, d):
+    """Whether `small_attention` holds a head's N keys and values of head dim d in its shared memory.  Above this cap
+    the camera head's token attention runs `token_attention`.  (Private: every public function of this module is a
+    launcher.)"""
+    return N <= 256 and (2 * N * d + 4 * N) * 4 <= 200 * 1024
+
+
 def small_attention(qkv, B, N, H, d):
-    if N > 256 or (2 * N * d + 4 * N) * 4 > 200 * 1024:
+    if not _small_attention_fits(N, d):
         raise ValueError(f"the camera head's token attention keeps all {N} views' keys and values of a head in shared memory "
                          f"(<= 256 views, <= {200 * 1024 // (8 * d + 16)} at head dim {d}); split the scene into fewer views per call")
     out = torch.empty((B * N, H * d), dtype=torch.float32, device=qkv.device)
     _call(qkv, "iggt_small_attention", 4.0 * B * N * N * H * d, 16.0 * B * N * H * d,
+          qkv.data_ptr(), out.data_ptr(), B, N, H, d, float(d) ** -0.5, _STREAM)
+    return out
+
+
+def token_attention(qkv, B, N, H, d):
+    """softmax(q k^T / sqrt(d)) v per scene and head for any number N of keys: qkv fp32 [B*N, 3*H*d] (q | k | v,
+    head-major inside each) -> fp32 [B*N, H*d].  Keys and values are streamed through shared memory, so N is bounded by
+    device memory only."""
+    if min(B, N, H) < 1:
+        raise ValueError(f"token_attention: B, N and H must be >= 1, got B={B} N={N} H={H}")
+    if d % 32 or not 32 <= d <= 128:
+        raise ValueError(f"token_attention: head dim {d} is not supported (a multiple of 32, at most 128)")
+    if B * N * 3 * H * d >= 1 << 63:
+        raise ValueError(f"token_attention: B*N*3*H*d = {B * N * 3 * H * d} elements does not fit a 64-bit index")
+    if -(-N // 16) > 65535:
+        raise ValueError(f"token_attention: {N} views per scene is more than the launch grid holds (<= {65535 * 16})")
+    if B * H > 2 ** 31 - 1:
+        raise ValueError(f"token_attention: B*H = {B * H} scene-heads is more than the launch grid holds (< 2^31)")
+    if (tuple(qkv.shape) != (B * N, 3 * H * d) or qkv.dtype != torch.float32 or not qkv.is_contiguous()
+            or qkv.data_ptr() % 16):
+        raise ValueError(f"token_attention: expected a contiguous, 16-byte aligned fp32 qkv of shape {(B * N, 3 * H * d)}, "
+                         f"got {qkv.dtype} {tuple(qkv.shape)}")
+    out = torch.empty((B * N, H * d), dtype=torch.float32, device=qkv.device)
+    _call(qkv, "iggt_token_attention", 4.0 * B * N * N * H * d, 16.0 * B * N * H * d,
           qkv.data_ptr(), out.data_ptr(), B, N, H, d, float(d) ** -0.5, _STREAM)
     return out
 

@@ -165,6 +165,15 @@ int iggt_skinny_gemm(const float* x, int64_t ldx, const void* W, int64_t ldw, co
 int iggt_small_attention(const float* qkv, float* out, int B, int N, int H, int d, float scale,
                          iggt_stream_t stream);
 
+/* fp32 softmax(q k^T * scale) v over any number N of keys per scene, same layout as iggt_small_attention
+ * (qkv[B*N, 3*H*d] -> out[B*N, H*d], each scene attends to its own N rows).  Keys and values are streamed through a
+ * fixed amount of shared memory with an online softmax, so N is bounded by device memory only (the camera tokens of
+ * scenes with more views than iggt_small_attention holds).  Deterministic: repeated calls are bit-identical.
+ * d: a multiple of 32, at most 128; qkv 16-byte aligned.  Returns -1 on bad arguments (B, N, H < 1, another d,
+ * ceil(N / 16) > 65535, B*N*3*H*d beyond int64) before any device work. */
+int iggt_token_attention(const float* qkv, float* out, int B, int N, int H, int d, float scale,
+                         iggt_stream_t stream);
+
 /* The whole camera head in ONE persistent launch (B*S <= 16 camera tokens; larger batches use iggt_skinny_gemm /
  * iggt_small_attention per layer).  Replaces iggt/heads/camera_head.py:83-154 (`CameraHead.forward` + `trunk_fn`:
  * token_norm, 4 x [embed_pose -> SiLU + Linear -> AdaLN modulate -> 4 Blocks(2048, 16 heads) -> trunk_norm ->
